@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the reference's headline metric (QPS of batched HNSW search at recall@10 >= 0.95) on B200.
+"""bench.py — the reference's headline metric (QPS of batched HNSW search at recall@10 >= 0.95) on an H100.
 
 One "step" = one batched `search()` over a fresh batch of synthetic queries against the index in HBM.
 Default workload = the configuration BASELINE.json's metric is quoted on: 10M x 768 f32 cosine (M=32, ef=128,
@@ -10,6 +10,7 @@ batch 4096, k=10). The collection is generated on the GPU and the graph is BUILT
   python bench.py --gpus 1 --steps K --warmup W            # our arm: CUDA path through the C ABI
   python bench.py --impl reference --steps K --warmup W    # the reference's own CPU search (oracle/_ref) of that graph
   torchrun ... bench.py --gpus N                           # N > 1: replicas (index fits one GPU) or shards (--parallelism)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as DIR/<name>.npy
 
 See DESIGN.md §6 for what each JSON key means and how the roofline figure is derived.
 """
@@ -80,6 +81,9 @@ def parse_args():
     p.add_argument("--cpu-sample-seconds", type=float, default=12.0)
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--no-next-rows", action="store_true")
+    p.add_argument("--dump-outputs", metavar="DIR",
+                   help="after the timed steps, write what the last one returned (keys, distances, counts, both counters) as "
+                        "DIR/<name>.npy in float64, so that two builds can be compared output for output on the same inputs")
     p.add_argument("--builder", default="gpu", choices=["gpu", "reference"],
                    help="who builds the graph both arms search: the GPU builder (default) or the reference on the host cores")
     p.add_argument("--parallelism", default=None, choices=["replica", "shard"],
@@ -261,12 +265,12 @@ def to_numpy_queries(a, q):
 
 
 # ------------------------------------------------------------------------------------------------
-#  clocks sampling (B200_PROFILING.md recipe)
+#  clocks sampling: the SM clock and its throttle reasons during the timed steps, with the card and its power limit
 # ------------------------------------------------------------------------------------------------
 
 class ClockSampler:
     FIELDS = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-              "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+              "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, gpu_index: int):
         self.samples = []
@@ -286,7 +290,7 @@ class ClockSampler:
     def _pump(self):
         for line in self.proc.stdout:
             parts = [p.strip() for p in line.split(",")]
-            if len(parts) >= 6 and parts[0].isdigit():
+            if len(parts) >= 7 and parts[0].isdigit():
                 self.samples.append(parts)
 
     def stop(self) -> dict:
@@ -303,7 +307,7 @@ class ClockSampler:
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for j, n in enumerate(names) if any(s[2 + j].lower().startswith("active") for s in self.samples)]
         return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": int(self.samples[0][1]), "reasons": reasons,
-                "samples": len(sm)}
+                "samples": len(sm), "power_limit_w": self.samples[0][6]}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -457,7 +461,7 @@ def run_b200_arm(a):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device — the GPU arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     os.environ["USEARCH_B200_DEVICE"] = str(local)
@@ -549,6 +553,11 @@ def run_b200_arm(a):
     barrier()
     if ncu_range:
         torch.cuda.profiler.stop()
+    if a.dump_outputs and rank == 0:  # the last timed step's results, still in the output buffers
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        for name, t in (("keys", keys_dev), ("distances", dist_dev), ("counts", cnt_dev), ("computed_distances", comp_dev),
+                        ("visited_members", vis_dev)):
+            np.save(os.path.join(a.dump_outputs, f"{name}.npy"), t.cpu().numpy().astype(np.float64))
     launches = index.kernel_launches - launches0
     elapsed_ms = ev0.elapsed_time(ev1)
     t = torch.tensor([elapsed_ms], device=device)
@@ -649,22 +658,9 @@ def run_b200_arm(a):
             next_rows = measure_next_rows(a, index, ref, queries[lo:lo + B], k, threads_all)
         del ref
 
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth (700 W card)"
     k_ms = float(np.mean(kernel_ms))
     achieved = float(np.mean(alg)) / (k_ms * 1e-3) / 1e9
-    traffic = None  # DRAM bytes per launch from an `ncu --set full` capture of this very workload at this N, else null
-    prof = os.path.join(ROOT, "profiles", "roofline_latest.json")
-    if os.path.exists(prof):
-        try:
-            pj = json.load(open(prof))
-            if pj.get("workload") == workload_name(a) and int(pj.get("n_gpus", 1)) == world and pj.get("parallelism", "replica") == a.parallelism:
-                traffic = pj.get("dram_bytes_per_launch")
-        except Exception:
-            pass
 
     # the metric is job throughput: queries answered per second. Replicas answer `world` different batches per step,
     # shards answer ONE batch per step between them.
@@ -679,7 +675,8 @@ def run_b200_arm(a):
         "vs_baseline": None, "dtype": a.dtype, "data": "synthetic",
         "config": {
             "workload": workload_name(a), "parallelism": parallelism, "queries_per_step": queries_per_step,
-            "l2_policy": "index (vectors+graph) larger than the 126 MB L2; every step uses a fresh query batch",
+            "l2_policy": "index (vectors+graph) larger than the 50 MB L2; every step uses a fresh query batch",
+            "gpu": torch.cuda.get_device_name(device),
             "index_hbm_gb": round(index.memory_usage / 1e9, 3), "index_build": info,
             "computed_distances_per_query": round(d_per_q, 1), "visited_members_per_query": round(h_per_q, 1),
         },
@@ -692,7 +689,7 @@ def run_b200_arm(a):
                 "note": ("usearch_b200_sharded_search_many" if shards > 1 else "usearch_search_many") +
                         " on pinned host buffers; H2D of queries and D2H of keys/distances/counts inside the timed call"},
         "roofline": {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-                     "frac": round(achieved / peak, 4), "traffic": traffic, "peak_source": peak_src,
+                     "frac": round(achieved / peak, 4), "peak_source": peak_src,
                      "kernel": "hnsw_search_kernel", "kernel_ms_per_launch": round(k_ms, 3),
                      "algorithmic_bytes_per_launch": int(np.mean(alg)),
                      "formula": "sum_q D_q*bytes_per_vector + H_q*(4+4*M0), D/H = the reference's computed_distances/visited_members; rank 0's launch"},

@@ -85,7 +85,7 @@ struct metric_punned_t {
                            : scalar_kind_ == usearch_scalar_f64_k ? 64 : 32;
         return (dimensions_ * bits + 7) / 8;
     }
-    char const* isa_name() const noexcept { return "sm_100a"; }
+    char const* isa_name() const noexcept { return "sm_90a"; }
     bool missing() const noexcept { return metric_kind_ == usearch_metric_unknown_k; }
 };
 

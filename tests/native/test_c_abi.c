@@ -55,7 +55,7 @@ int main(int argc, char** argv) {
     EXPECT(!error);
     EXPECT(usearch_size(index, &error) > 0 && usearch_dimensions(index, &error) == dims);
     EXPECT(usearch_connectivity(index, &error) >= 2);
-    EXPECT(strcmp(usearch_hardware_acceleration(index, &error), "sm_100a") == 0);
+    EXPECT(strcmp(usearch_hardware_acceleration(index, &error), "sm_90a") == 0);
     EXPECT(usearch_memory_usage(index, &error) > 0);
 
     /* single-query searches, one call per query like Go / C# callers (golang/lib.go:628) */

@@ -59,7 +59,7 @@ def test_init_and_metadata_without_gpu():
         Index.metadata(np.zeros(200, dtype=np.uint8))
     index = Index(ndim=64, metric="cos", dtype="f32", connectivity=16, expansion_search=77)
     assert index.ndim == 64 and index.connectivity == 16 and index.expansion_search == 77 and index.size == 0
-    assert index.hardware_acceleration == "sm_100a"
+    assert index.hardware_acceleration == "sm_90a"
     import torch
     if not torch.cuda.is_available():  # mutation needs the device just like search does: no CPU fallback
         with pytest.raises(RuntimeError, match="no CPU fallback"):

@@ -151,9 +151,9 @@ def test_cluster_matches_reference(metric, scalar, n, d, m):
 
 
 
-@pytest.mark.parametrize("kernel", ["imma", "umma", "tiled"])
+@pytest.mark.parametrize("kernel", ["imma", "wgmma", "tiled"])
 def test_i8_exact_kernels_agree_with_the_reference(kernel):
-    """The three i8 scans — tcgen05 with TMEM accumulators (default), mma.sync, dp4a — forced one at a time
+    """The three i8 scans — wgmma with TMA operand loads (default), mma.sync, dp4a — forced one at a time
     (USEARCH_B200_EXACT is read once per process, hence the subprocess): same bits, index mode and free function."""
     import os
     import subprocess

@@ -1,5 +1,5 @@
 """Large-index check: a vector slab beyond 4 GiB, so every byte offset on the device and in the loader must be
-64-bit (about 20 s on a B200 box; skipped when the host has less than 32 GB free, USEARCH_B200_LARGE=0 disables). The graph is synthetic (random links over three levels) — the traversal
+64-bit (skipped when the host has less than 32 GB free, USEARCH_B200_LARGE=0 disables). The graph is synthetic (random links over three levels) — the traversal
 does not need a navigable graph to be compared decision for decision with the oracle."""
 import os
 

@@ -181,7 +181,7 @@ void usearch_free(usearch_index_t index, usearch_error_t*) { delete as_index(ind
 
 size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { return as_index(index)->hbm_bytes; }
 
-char const* usearch_hardware_acceleration(usearch_index_t, usearch_error_t*) { return "sm_100a"; }
+char const* usearch_hardware_acceleration(usearch_index_t, usearch_error_t*) { return "sm_90a"; }
 
 size_t usearch_serialized_length(usearch_index_t index, usearch_error_t*) { return as_index(index)->serialized_length(); }
 

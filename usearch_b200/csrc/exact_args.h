@@ -1,5 +1,5 @@
 /*
- *  exact_args.h — launch arguments shared by the exact-search kernels (exact_kernel.cu, exact_imma.cu).
+ *  exact_args.h — launch arguments shared by the exact-search kernels (exact_kernel.cu, exact_imma.cu, exact_wgmma.cu).
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -35,11 +35,11 @@ int exact_imma_tile_vectors();
 cudaError_t exact_imma_self_dots(uint8_t const* rows, uint64_t stride, uint32_t chunks16, uint32_t count, int* out, cudaStream_t stream);
 cudaError_t exact_imma_launch(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, cudaStream_t stream);
 
-/* exact_umma.cu: the same scan on tcgen05 (TMEM accumulators, TMA operand loads) */
-size_t exact_umma_smem_bytes();
-int exact_umma_tile_queries();
-int exact_umma_tile_vectors();
-bool exact_umma_usable(device_index_t const& ix, exact_args_t const& a);
-cudaError_t exact_umma_launch(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, cudaStream_t stream);
+/* exact_wgmma.cu: the same scan on warpgroup MMAs (wgmma, TMA operand loads) */
+size_t exact_wgmma_smem_bytes();
+int exact_wgmma_tile_queries();
+int exact_wgmma_tile_vectors();
+bool exact_wgmma_usable(device_index_t const& ix, exact_args_t const& a);
+cudaError_t exact_wgmma_launch(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, cudaStream_t stream);
 
 } // namespace usearch_b200

@@ -1,6 +1,6 @@
 /*
  *  exact_i8.cuh — the three i8 metrics as functions of the integer triple (ab, a2, b2), shared by the tensor-core scans
- *  (exact_imma.cu: mma.sync; exact_umma.cu: tcgen05):
+ *  (exact_imma.cu: mma.sync; exact_wgmma.cu: wgmma):
  *      ip    1 - float(ab)                               index_plugins.hpp:1914-1916 over simsimd_dot_i8
  *      l2sq  float(a2 + b2 - 2 ab)  == sum (a-b)^2       spatial.h l2sq_i8 (i32 accumulation)
  *      cos   normalise(float(ab), float(a2), float(b2))  spatial.h:1904-1972 -> the f32 normaliser

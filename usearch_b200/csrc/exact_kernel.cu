@@ -435,30 +435,30 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     size_t const tiled_smem = ((size_t)qpc_tiled * ix.vec_stride + 16 + 127) / 128 * 128 + 2 * (size_t)tile_vectors * a.stage_stride;
     static int const forced = [] {
         char const* v = std::getenv("USEARCH_B200_EXACT");
-        return !v ? 0 : (std::strcmp(v, "scan") == 0 ? 1 : (std::strcmp(v, "tiled") == 0 ? 2 : (std::strcmp(v, "imma") == 0 ? 3 : (std::strcmp(v, "umma") == 0 ? 4 : 0))));
+        return !v ? 0 : (std::strcmp(v, "scan") == 0 ? 1 : (std::strcmp(v, "tiled") == 0 ? 2 : (std::strcmp(v, "imma") == 0 ? 3 : (std::strcmp(v, "wgmma") == 0 ? 4 : 0))));
     }();
     /* i8: integer sums are order independent, the tensor cores give the reference's bits (exact_imma.cu) */
     bool const imma = !big_k && ix.scalar == SCALAR_I8 && (forced == 0 || forced == 3 || forced == 4) &&
                       (ix.metric == METRIC_IP || ix.metric == METRIC_L2SQ || ix.metric == METRIC_COS);
     if ((forced == 3 || forced == 4) && !imma) return "The tensor-core exact-search kernels serve i8 vectors only";
-    /* tcgen05 (exact_umma.cu) when the driver can encode tensor maps; mma.sync (exact_imma.cu) otherwise or when forced */
-    bool const umma = imma && forced != 3 && exact_umma_usable(ix, a); /* count <= 24; larger counts stay on mma.sync */
+    /* wgmma (exact_wgmma.cu) when the driver can encode tensor maps; mma.sync (exact_imma.cu) otherwise or when forced */
+    bool const wgmma = imma && forced != 3 && exact_wgmma_usable(ix, a); /* count <= 24; larger counts stay on mma.sync */
     bool const tiled = !imma && (forced == 1 && !big_k ? false : tiled_smem <= 227 * 1024);
     if (big_k && !tiled) return "Exact search with count > 256 needs vectors that fit the tiled stage";
     if (forced == 2 && !tiled) return "Vectors too long for the tiled exact-search stage";
-    int const vpp = umma ? exact_umma_tile_vectors() : (imma ? exact_imma_tile_vectors() : (tiled ? tile_vectors : 32 / lpv)); /* vectors per tile */
-    uint32_t const qpc = umma ? (uint32_t)exact_umma_tile_queries()
+    int const vpp = wgmma ? exact_wgmma_tile_vectors() : (imma ? exact_imma_tile_vectors() : (tiled ? tile_vectors : 32 / lpv)); /* vectors per tile */
+    uint32_t const qpc = wgmma ? (uint32_t)exact_wgmma_tile_queries()
                               : (imma ? (uint32_t)exact_imma_tile_queries() : (tiled ? (uint32_t)qpc_tiled : (uint32_t)EXACT_WARPS));
     uint32_t off = qpc * (uint32_t)ix.vec_stride;
     a.off_queries = 0;
     a.off_bars = off;
     off = (off + 16 + 127) / 128 * 128;
     a.off_stage = off;
-    size_t const smem = umma ? exact_umma_smem_bytes() : (imma ? exact_imma_smem_bytes() : off + 2 * (size_t)vpp * a.stage_stride);
+    size_t const smem = wgmma ? exact_wgmma_smem_bytes() : (imma ? exact_imma_smem_bytes() : off + 2 * (size_t)vpp * a.stage_stride);
     if (smem > 227 * 1024) return "Vectors too long for the exact-search stage";
     uint32_t const groups = (uint32_t)((nq + qpc - 1) / qpc);
     /* cut the dataset so that the grid fills whole waves of the resident CTAs (1 per SM tiled, ~3 per SM otherwise) */
-    uint32_t const resident = (uint32_t)sm_count * (umma ? 1u : (imma ? 2u : (tiled ? 1u : 3u)));
+    uint32_t const resident = (uint32_t)sm_count * (wgmma ? 1u : (imma ? 2u : (tiled ? 1u : 3u)));
     uint32_t const max_segments = std::max<uint32_t>(1, std::min<uint32_t>((ix.n + 8 * (uint32_t)vpp - 1) / (8 * (uint32_t)vpp), 65535u));
     uint32_t segments = 1;
     {
@@ -500,7 +500,7 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     a.out_counts = d_counts;
     dim3 const grid(groups, segments);
     cudaError_t e = cudaErrorInvalidValue;
-    if (umma) e = exact_umma_launch(ix, a, swap, grid, stream);
+    if (wgmma) e = exact_wgmma_launch(ix, a, swap, grid, stream);
     else if (imma) e = exact_imma_launch(ix, a, swap, grid, stream);
     else switch (ix.scalar) {
     case SCALAR_F32:

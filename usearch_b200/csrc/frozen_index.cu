@@ -103,7 +103,7 @@ char const* frozen_index_t::ensure_context() {
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
         cudaGetLastError();
-        return "No CUDA device: the B200 search backend has no CPU fallback";
+        return "No CUDA device: the GPU search backend has no CPU fallback";
     }
     CU(cudaSetDevice(device));
     if (!stream) {
@@ -153,7 +153,7 @@ char const* frozen_index_t::load_blob(uint8_t const* blob, size_t length) {
     p += 64;
     (void)count_present;
     if (!search_supported(head_metric, head_scalar))
-        return "This metric / scalar kind has no sm_100a kernel and the backend has no CPU fallback";
+        return "This metric / scalar kind has no sm_90a kernel and the backend has no CPU fallback";
     size_t const bpv = (dims * bits_per_scalar(head_scalar) + 7) / 8;
     if (rows && cols != bpv) return "Matrix columns do not match bytes per vector";
 
@@ -945,7 +945,7 @@ char const* frozen_index_t::exact_host(void const* q, size_t nq, size_t stride, 
 char const* exact_search_free(void const* dataset, size_t n, size_t dataset_stride, void const* queries_h, size_t nq, size_t queries_stride,
                               uint32_t scalar, size_t dimensions, uint32_t metric, size_t k, uint64_t* keys, size_t keys_stride,
                               float* distances, size_t distances_stride) {
-    if (!search_supported(metric, scalar)) return "This metric / scalar kind has no sm_100a kernel and the backend has no CPU fallback";
+    if (!search_supported(metric, scalar)) return "This metric / scalar kind has no sm_90a kernel and the backend has no CPU fallback";
     if (!nq || !k) return nullptr;
     if (k > n) return "More neighbours requested than the dataset holds";
     if (n >= 0xFFFFFFFFull) return "Too many entries for 32-bit slots";

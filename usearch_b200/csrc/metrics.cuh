@@ -44,36 +44,6 @@ template <int LPV> __device__ __forceinline__ int reduce_add_i32(int v) {
     return v;
 }
 
-/* ---- packed f32 pairs: Blackwell issues two IEEE fma.rn.f32 in one FFMA2 -------------------- */
-/*
- *  `fma.rn.f32x2` / `sub.rn.f32x2` (sm_100: SASS FFMA2 / FADD2) apply the scalar round-to-nearest operation to both halves
- *  of a 64-bit register pair. Every accumulator still sees the same operands in the same order, so the sums keep the bits
- *  of the scalar chains they replace (asserted by every parity test). Used by the WORD half-precision metrics, where one
- *  FFMA2 per 32-bit word replaces two scalar fmas (10M x 768 f16: 208 -> 191 ms per 65536 queries together with the log
- *  cleaning). NOT used by the f32 metrics: there it turns four independent fma chains per lane into two, and with one warp
- *  per scheduler the longer dependency distance costs more than the halved instruction count saves (measured at 10M x 768
- *  f32: distance phase 1.60 M -> 1.96 M cycles per query).
- */
-__device__ __forceinline__ unsigned long long pack2(uint32_t lo, uint32_t hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-    return r;
-}
-__device__ __forceinline__ unsigned long long pack2f(float lo, float hi) { return pack2(__float_as_uint(lo), __float_as_uint(hi)); }
-__device__ __forceinline__ void unpack2f(unsigned long long v, float& lo, float& hi) {
-    uint32_t a, b;
-    asm("mov.b64 {%0, %1}, %2;" : "=r"(a), "=r"(b) : "l"(v));
-    lo = __uint_as_float(a);
-    hi = __uint_as_float(b);
-}
-__device__ __forceinline__ void fma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
-}
-__device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
 /* ---- f32 -------------------------------------------------------------------------------- */
 
 __device__ __forceinline__ float reduce16_f32(float const v[4]) {
@@ -349,21 +319,18 @@ template <class C> struct l2sq_halfw_t {
     static constexpr bool NORMS = false;
     using unit_t = uint32_t;
     template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
-    struct acc_t { unsigned long long p; };
+    struct acc_t { float v[2]; };
     struct qconst_t {};
-    static __device__ __forceinline__ void init(acc_t& a) { a.p = 0ull; }
+    static __device__ __forceinline__ void init(acc_t& a) { a.v[0] = a.v[1] = 0.f; }
     static __device__ __forceinline__ void step(acc_t& a, uint32_t b, uint32_t q) {
         float b0, b1, q0, q1;
         C::widen(b, b0, b1);
         C::widen(q, q0, q1);
-        unsigned long long const x = sub2(pack2f(q0, q1), pack2f(b0, b1));
-        fma2(a.p, x, x);
+        float const x0 = __fsub_rn(q0, b0), x1 = __fsub_rn(q1, b1);
+        a.v[0] = __fmaf_rn(x0, x0, a.v[0]);
+        a.v[1] = __fmaf_rn(x1, x1, a.v[1]);
     }
-    static __device__ __forceinline__ float finish(acc_t const& a, qconst_t) {
-        float v[2];
-        unpack2f(a.p, v[0], v[1]);
-        return reduce_words_f64(v);
-    }
+    static __device__ __forceinline__ float finish(acc_t const& a, qconst_t) { return reduce_words_f64(a.v); }
     static __device__ __forceinline__ qconst_t prepare(uint4 const*, uint32_t, int) { return {}; }
 };
 
@@ -372,18 +339,18 @@ template <class C> struct ip_halfw_t {
     static constexpr bool NORMS = false;
     using unit_t = uint32_t;
     template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
-    struct acc_t { unsigned long long p; };
+    struct acc_t { float v[2]; };
     struct qconst_t {};
-    static __device__ __forceinline__ void init(acc_t& a) { a.p = 0ull; }
+    static __device__ __forceinline__ void init(acc_t& a) { a.v[0] = a.v[1] = 0.f; }
     static __device__ __forceinline__ void step(acc_t& a, uint32_t b, uint32_t q) {
         float b0, b1, q0, q1;
         C::widen(b, b0, b1);
         C::widen(q, q0, q1);
-        fma2(a.p, pack2f(q0, q1), pack2f(b0, b1));
+        a.v[0] = __fmaf_rn(q0, b0, a.v[0]);
+        a.v[1] = __fmaf_rn(q1, b1, a.v[1]);
     }
     static __device__ __forceinline__ float finish(acc_t const& a, qconst_t) {
-        float v[2];
-        unpack2f(a.p, v[0], v[1]);
+        float const* v = a.v;
         return __fsub_rn(1.0f, reduce_words_f64(v));
     }
     static __device__ __forceinline__ qconst_t prepare(uint4 const*, uint32_t, int) { return {}; }
@@ -393,18 +360,18 @@ template <class C> struct cos_halfw_t {
     static constexpr int LPV = 4, UPC = 4;
     static constexpr bool NORMS = true;
     using unit_t = uint32_t;
-    struct acc_t { unsigned long long p; };
+    struct acc_t { float v[2]; };
     using qconst_t = typename cos_half_t<C>::qconst_t;
-    static __device__ __forceinline__ void init(acc_t& a) { a.p = 0ull; }
+    static __device__ __forceinline__ void init(acc_t& a) { a.v[0] = a.v[1] = 0.f; }
     static __device__ __forceinline__ void step(acc_t& a, uint32_t b, uint32_t q) {
         float b0, b1, q0, q1;
         C::widen(b, b0, b1);
         C::widen(q, q0, q1);
-        fma2(a.p, pack2f(q0, q1), pack2f(b0, b1));
+        a.v[0] = __fmaf_rn(q0, b0, a.v[0]);
+        a.v[1] = __fmaf_rn(q1, b1, a.v[1]);
     }
     static __device__ __forceinline__ float finish(acc_t const& a, qconst_t) {
-        float v[2];
-        unpack2f(a.p, v[0], v[1]);
+        float const* v = a.v;
         return reduce_words_f64(v);
     }
     static __device__ __forceinline__ float finalize(float ab, qconst_t qc, float b2) { return cos_normalize_f32(ab, qc.a2, b2); }

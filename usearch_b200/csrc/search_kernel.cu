@@ -949,13 +949,13 @@ cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStr
 /* ---- host-side dispatch --------------------------------------------------------------------- */
 
 /*
- *  Which kernel serves which index (measured on B200, profiles/r02_variants.md):
+ *  Which kernel serves which index:
  *    f32, vectors >= 256 B      STAGED, 4 lanes per vector, 8 resident warps per SM allowed by the register budget
  *    f16 / bf16, >= 256 B       STAGED with the WORD metrics (4 lanes per vector split by accumulator) compiled for 16
- *                               resident warps per SM; one stage set up to 2 KB vectors (1M x 768 f16, ef 256: 0.40 ->
- *                               0.61 of the HBM peak against one lane per vector in a single 32-slot set)
- *    i8, >= 256 B               STAGED compiled for 16 resident warps per SM, one stage set up to 2 KB (1M x 1024 i8:
- *                               0.53 -> 0.64): a hop moves few bytes, so resident warps matter more than double buffering
+ *                               resident warps per SM; one stage set up to 2 KB vectors (a quarter of the shared memory
+ *                               per warp of one lane per vector in a single 32-slot set)
+ *    i8, >= 256 B               STAGED compiled for 16 resident warps per SM, one stage set up to 2 KB: a hop moves few
+ *                               bytes, so resident warps matter more than double buffering
  *    b1, and anything < 256 B   DIRECT (16-byte chunks through registers)
  *  Every one of them also exists as an INSERT-mode kernel for the builder.
  */

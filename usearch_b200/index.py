@@ -64,7 +64,7 @@ def load_library() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                          "(nvcc, sm_100a). The B200 backend has no CPU fallback.")
+                          "(nvcc, sm_90a). The GPU backend has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     err = C.POINTER(C.c_char_p)
     lib.usearch_version.restype = C.c_char_p
