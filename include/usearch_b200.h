@@ -254,10 +254,12 @@ size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries
 /* Phase introspection of the search kernel: enable != 0 turns on (and zeroes) sixteen device-side
  * counters summed over all queries since; `counters16` (may be NULL) first receives the current values:
  * cycles of setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay |
- * output, then queries | heap pushes | sum of per-query max heap size | max heap size | 5 reserved. */
+ * output, then queries | heap pushes | sum of per-query max heap size | max heap size | candidates prefiltered (layer-0
+ * candidates of cos / ip f32 judged on their int8 shadow) | survivors (those of them whose f32 row was read) | 3 reserved. */
 void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16);
-/* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm"); results
- * never depend on them. Returns 0, or -1 for an unknown knob. */
+/* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
+ * candidates of cos / ip f32 on their int8 shadow first, on by default); results never depend on them. Returns 0, or -1
+ * for an unknown knob. */
 int usearch_b200_tune(usearch_index_t index, char const* knob, int value);
 int usearch_b200_device(usearch_index_t index);
 uint64_t usearch_b200_kernel_launches(usearch_index_t index);

@@ -55,14 +55,14 @@ def main():
     stream = torch.cuda.Stream(device)
     torch.cuda.synchronize(device)
     torch.cuda.set_stream(stream)
-    peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+    peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
     R = min(B, 1024)
     gt, _ = bench.exact_topk_gpu(a, coll, q_dev[:R], k)
     gt = gt.cpu().numpy().astype(np.uint64)
     m0 = 2 * index.connectivity
     print(json.dumps({"workload": bench.workload_name(a), "build_s": round(build_s, 1), "hbm_gb": round(index.memory_usage / 1e9, 2)}), flush=True)
     for spec in o.configs.split(";"):
-        knobs = {"stage_sets": 0, "warps_per_sm": 0}
+        knobs = {"stage_sets": 0, "warps_per_sm": 0, "prefilter": 1}
         if spec != "base":
             for kv in spec.split(","):
                 name, value = kv.split("=")
@@ -91,7 +91,15 @@ def main():
         line = {"config": spec, "kernel_ms": round(k_ms, 3), "qps": round(B / (k_ms * 1e-3)), "alg_gbs": round(gbs, 1), "frac": round(gbs / peak, 4),
                 "recall_at_10": round(rec, 4)}
         if o.phases:
-            line["phases"] = {k2: round(v, 1) for k2, v in index.profile_phases(False).items()}
+            ph = index.profile_phases(False)
+            line["phases"] = {k2: round(v, 1) for k2, v in ph.items()}
+            # bytes the kernel moved per query: the vectors it read, the codes and records of prefiltered candidates, the
+            # lists of the hops (the algorithmic figure counts a full row for every computed distance instead)
+            d_q, h_q = float(comp.sum(dtype=torch.int64).item()) / B, float(vis.sum(dtype=torch.int64).item()) / B
+            exact = d_q - ph["prefiltered"] + ph["survivors"]
+            code = (a.dim + 15) // 16 * 16 + 16
+            line["physical_bytes_per_query"] = round(exact * index.bytes_per_vector + ph["prefiltered"] * code + h_q * (4 + 4 * m0))
+            line["algorithmic_bytes_per_query"] = round(d_q * index.bytes_per_vector + h_q * (4 + 4 * m0))
         print(json.dumps(line), flush=True)
 
 

@@ -565,6 +565,7 @@ char const* frozen_index_t::reserve_slots(size_t slots) {
         ix.chunks16 = (uint32_t)(ix.vec_stride / 16);
         ix.metric = metric;
         ix.scalar = scalar;
+        if (search_needs_shadow(ix)) ix.code_stride = search_code_stride(ix);
         d = ix;
         loaded = true;
     }
@@ -587,8 +588,13 @@ char const* frozen_index_t::reserve_slots(size_t slots) {
         if (char const* e = regrow<uint32_t>(dev_allocs[5], d.deleted_bits, (old_cap + 31) / 32, (slots + 31) / 32, 0, stream)) return e;
     if (search_needs_norms(metric, scalar))
         if (char const* e = regrow<float>(dev_allocs[6], d.norms, old_cap, slots, -1, stream)) return e;
+    if (d.code_stride) { /* the int8 shadow of cos / ip f32 (prefilter_bound.h) */
+        if (char const* e = regrow<int8_t>(dev_allocs[8], d.codes, old_cap * d.code_stride, slots * d.code_stride, -1, stream)) return e;
+        if (char const* e = regrow<pf_record_t>(dev_allocs[9], d.shadow, old_cap, slots, -1, stream)) return e;
+    }
     capacity = slots;
-    hbm_bytes = capacity * (d.vec_stride + 8 + (size_t)d.m0_stride * 4 + 4 + (d.norms ? 4 : 0)) + upper_capacity * d.m_stride * 4 +
+    hbm_bytes = capacity * (d.vec_stride + 8 + (size_t)d.m0_stride * 4 + 4 + (d.norms ? 4 : 0) +
+                            (d.code_stride ? d.code_stride + sizeof(pf_record_t) : 0)) + upper_capacity * d.m_stride * 4 +
                 (d.deleted_bits ? (capacity + 31) / 32 * 4 : 0);
     visited_zeroed_words = 0; /* the visits bitmaps are sized by capacity */
     return nullptr;
@@ -682,6 +688,13 @@ char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vecto
         part.vectors = slab;
         part.n = (uint32_t)count;
         CU(search_compute_norms(part, const_cast<float*>(d.norms) + first, stream));
+    }
+    if (d.codes) { /* after the norms: the records copy them */
+        device_index_t part = d;
+        part.vectors = slab;
+        part.n = (uint32_t)count;
+        CU(search_compute_shadow(part, d.norms ? d.norms + first : nullptr, const_cast<int8_t*>(d.codes) + first * d.code_stride,
+                                 const_cast<pf_record_t*>(d.shadow) + first, stream));
     }
     CU(cudaStreamSynchronize(stream)); /* `vectors` / `new_keys` may be pageable host memory owned by the caller */
 

@@ -567,6 +567,7 @@ int usearch_b200_tune(usearch_index_t index, char const* knob, int value) {
     std::lock_guard<std::mutex> lock(ix->mutex);
     if (!std::strcmp(knob, "stage_sets")) ix->tune.stage_sets = value;
     else if (!std::strcmp(knob, "warps_per_sm")) ix->tune.warps_per_sm = value;
+    else if (!std::strcmp(knob, "prefilter")) ix->tune.prefilter = value;
     else return -1;
     return 0;
 }

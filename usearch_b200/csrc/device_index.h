@@ -16,6 +16,9 @@
  *    upper        [rows x m_stride] u32    rows level 1..L of every multi-level node, back to back
  *    norms        [n] f32                  cos/f32 only: squared norm of every vector, accumulated by
  *                                          the exact fma chain the metric would use per distance
+ *    codes        [n x code_stride] i8     cos/ip f32 served by the STAGED kernel: the int8 shadow of every vector
+ *                                          (prefilter_bound.h), code_stride = round_up(dims, 16), zero padding
+ *    shadow       [n] 16-byte records      the same indexes: scale, residual bound, norm bound, squared norm
  *    deleted_bits [ceil(n/32)] u32         bit set when keys[slot] == free_key; NULL when the
  *                                          index holds no removed entries (the common case), which
  *                                          removes the per-candidate key read of
@@ -26,6 +29,8 @@
 #include <cstdint>
 
 namespace usearch_b200 {
+
+struct pf_record_t; /* prefilter_bound.h */
 
 constexpr uint32_t EMPTY_SLOT = 0xFFFFFFFFu;
 constexpr uint32_t SNAN_BITS = 0x7FA00000u; /* numeric_limits<float>::signaling_NaN, index.hpp:2715-2720 */
@@ -45,6 +50,9 @@ struct device_index_t {
     uint32_t const* upper = nullptr;
     uint32_t const* deleted_bits = nullptr;
     float const* norms = nullptr; /* [n] ||v||^2 in the metric's own summation order (cos f32), else NULL */
+    int8_t const* codes = nullptr;        /* [n x code_stride] int8 shadow (cos / ip f32, STAGED), else NULL */
+    pf_record_t const* shadow = nullptr; /* [n] its records */
+    uint32_t code_stride = 0;             /* bytes */
     uint64_t vec_stride = 0; /* bytes */
     uint32_t n = 0;
     uint32_t m0 = 0, m0_stride = 0; /* connectivity_base and its row stride (u32 units, multiple of 4) */
@@ -110,8 +118,13 @@ struct search_args_t {
      * that the 4-lane groups of a quarter-warp read disjoint banks) */
     uint32_t off_bars = 0, off_stage = 0, stage_stride = 0;
     uint32_t stage_sets = 1; /* 2 = double buffered: 2 x (32/LPV) slots, the next pass lands during the math */
+    /* layer-0 prefilter (cos / ip f32 with a shadow): once `top` is full, a hop first bulk-copies the int8 codes of its
+     * candidates into the stage area (`code_pass` per pass, `code_smem_stride` bytes apart), rejects those whose lower
+     * bound proves d >= radius, and measures only the survivors (listed in surv_s / surv_i, exact values in surv_d) */
+    uint32_t prefilter = 0, code_pass = 0, code_smem_stride = 0, off_surv_s = 0, off_surv_i = 0, off_surv_d = 0;
     /* optional introspection: 8 cycle counters summed over all queries (lane 0 clock64 deltas):
-     * setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay | output */
+     * setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay | output, then counts
+     * (include/usearch_b200.h, usearch_b200_profile_phases) */
     unsigned long long* phase_cycles = nullptr;
 };
 

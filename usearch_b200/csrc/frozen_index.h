@@ -32,6 +32,10 @@ int search_max_warps_per_sm(device_index_t const& ix);
 bool search_single_stage_set(device_index_t const& ix);
 bool search_needs_norms(uint32_t metric, uint32_t scalar);
 cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStream_t stream);
+bool search_needs_shadow(device_index_t const& ix);
+uint32_t search_code_stride(device_index_t const& ix);
+cudaError_t search_compute_shadow(device_index_t const& ix, float const* norms, int8_t* codes, pf_record_t* records,
+                                  cudaStream_t stream);
 cudaError_t search_fill_empty(uint64_t* keys, float* dists, uint32_t* counts, uint32_t* computed, uint32_t* visited, size_t nq,
                               size_t k, cudaStream_t stream);
 cudaError_t search_build_allow_bits(device_index_t const& ix, uint64_t const* allowed_sorted, uint32_t m, uint32_t* bits,
@@ -49,6 +53,7 @@ struct launch_plan_t {
     size_t visited_words_per_warp() const { return visited_bitmap_words ? visited_bitmap_words : visited_cap; }
     uint32_t smem_per_warp = 0, off_top_d = 0, off_top_s = 0, off_cand_s = 0, off_cand_d = 0, off_heap = 0;
     uint32_t off_bars = 0, off_stage = 0, stage_stride = 0, stage_sets = 1;
+    uint32_t off_surv_s = 0, off_surv_i = 0, off_surv_d = 0, code_pass = 0, code_smem_stride = 0; /* prefilter */
     int blocks = 0;
     uint32_t warps_per_sm_target = 0;
     size_t smem_per_block = 0;
@@ -140,13 +145,14 @@ struct frozen_index_t {
     device_index_t d;
     size_t hbm_bytes = 0;
     bool loaded = false;
-    void* dev_allocs[8] = {nullptr};
+    void* dev_allocs[10] = {nullptr}; /* vectors keys nbr0 upper_base upper deleted norms - codes shadow */
 
     /* tuning knobs of the search launch: environment at construction (USEARCH_B200_STAGE_SETS, _WARPS_PER_SM),
      * changeable per handle with usearch_b200_tune (bench sweeps, tests) */
     struct tune_t {
         int stage_sets = env_int("USEARCH_B200_STAGE_SETS", 0);     /* 0 = planned, 1 or 2 = forced */
         int warps_per_sm = env_int("USEARCH_B200_WARPS_PER_SM", 0); /* 0 = as many as fit, else an upper bound */
+        int prefilter = env_int("USEARCH_B200_PREFILTER", 1);       /* 0 = measure every layer-0 candidate exactly */
         static int env_int(char const* name, int fallback) {
             char const* v = std::getenv(name);
             return v ? std::atoi(v) : fallback;

@@ -26,6 +26,7 @@
 #include <cuda_runtime.h>
 
 #include "device_index.h"
+#include "prefilter_bound.h"
 
 namespace usearch_b200 {
 
@@ -98,6 +99,11 @@ struct l2sq_f32_t {
 struct ip_f32_t {
     static constexpr int LPV = 4;
     static constexpr bool NORMS = false;
+    /* layer-0 prefilter through the int8 shadow (search_kernel.cu, measure_prefiltered; bound: prefilter_bound.h) */
+    static constexpr bool PREFILTER = true;
+    static __device__ __forceinline__ double pf_lower(float dot, pf_record_t r, float a2, uint32_t n) {
+        return pf_ip_lower(dot, r.s, r.rho, a2, r.bnorm, n);
+    }
     template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
     template <class Q> static __device__ __forceinline__ float finalize_sw(float raw, Q, float) { return raw; }
     struct acc_t { float v[4]; };
@@ -123,6 +129,10 @@ struct ip_f32_t {
 struct cos_f32_t {
     static constexpr int LPV = 4;
     static constexpr bool NORMS = true;
+    static constexpr bool PREFILTER = true; /* see ip_f32_t */
+    static __device__ __forceinline__ double pf_lower(float dot, pf_record_t r, float a2, uint32_t n) {
+        return pf_cos_lower(dot, r.s, r.rho, a2, r.b2, n);
+    }
     struct acc_t { float ab[4]; };
     struct qconst_t { float a2; };
     static __device__ __forceinline__ void init(acc_t& a) { a.ab[0] = a.ab[1] = a.ab[2] = a.ab[3] = 0.f; }
@@ -388,6 +398,14 @@ template <class M, class = void> struct unit_of {
 template <class M> struct unit_of<M, decltype((void)sizeof(typename M::unit_t), void())> {
     using type = typename M::unit_t;
     static constexpr uint32_t UPC = (uint32_t)M::UPC;
+};
+
+/* M::PREFILTER where the metric declares it, else false: every other metric keeps the plain search */
+template <class M, class = void> struct prefilter_of {
+    static constexpr bool value = false;
+};
+template <class M> struct prefilter_of<M, decltype((void)M::PREFILTER, void())> {
+    static constexpr bool value = M::PREFILTER;
 };
 
 /* ---- i8 --------------------------------------------------------------------------------- */

@@ -330,7 +330,8 @@ __device__ __noinline__ void measure_direct(device_index_t const& ix, warp_ctx_t
  */
 template <class M>
 __device__ __forceinline__ void measure_staged(device_index_t const& ix, search_args_t const& a, warp_ctx_t& w,
-                                               typename M::qconst_t qc, uint32_t ncand, int lane) {
+                                               typename M::qconst_t qc, uint32_t ncand, int lane, uint32_t const* slots,
+                                               float* out) {
     constexpr int LPV = M::LPV, VPP = 32 / LPV;
     int const g = lane / LPV, sub = lane % LPV;
     bool const two_sets = a.stage_sets > 1;
@@ -340,7 +341,7 @@ __device__ __forceinline__ void measure_staged(device_index_t const& ix, search_
      * loop; lane 0 issuing all copies back to back measured 7 % slower end to end (round 1). */
     auto issue = [&](uint32_t pass) {
         uint32_t const base = pass * VPP, cnt = min((uint32_t)VPP, ncand - base), set = two_sets ? (pass & 1u) : 0u;
-        uint32_t const my_slot = (uint32_t)lane < cnt ? w.cand_s[base + lane] : 0u;
+        uint32_t const my_slot = (uint32_t)lane < cnt ? slots[base + lane] : 0u;
         uint32_t const bar = w.bars_addr + 8u * set;
         if (lane == 0) mbar_expect_tx(bar, cnt * bytes);
         __syncwarp();
@@ -392,7 +393,7 @@ __device__ __forceinline__ void measure_staged(device_index_t const& ix, search_
             for (; j < u1; j += LPV) M::step(acc, buf[j], qu[j]);
         }
         float const d = M::finish(acc, qc); /* horizontal reduce (warp-wide shuffles: every lane) */
-        if (act && sub == 0) w.cand_d[base + g] = d;
+        if (act && sub == 0) out[base + g] = d;
         w.phase ^= 1u << set; /* one parity bit per set */
         __syncwarp();         /* every lane is done with this set before it is refilled */
         uint32_t const next = pass + (two_sets ? 2u : 1u);
@@ -412,7 +413,7 @@ __device__ __forceinline__ void measure_list(device_index_t const& ix, search_ar
         if ((uint32_t)lane < ncand) n0 = __ldg(ix.norms + w.cand_s[lane]);
         if ((uint32_t)lane + 32 < ncand) n1 = __ldg(ix.norms + w.cand_s[lane + 32]);
     }
-    if constexpr (STAGED) measure_staged<M>(ix, a, w, qc, ncand, lane);
+    if constexpr (STAGED) measure_staged<M>(ix, a, w, qc, ncand, lane, w.cand_s, w.cand_d);
     else measure_direct<M>(ix, w, qc, ncand, lane);
     if constexpr (M::NORMS) { /* one candidate per lane: a single f64 normalisation sequence per hop */
         if ((uint32_t)lane < ncand) w.cand_d[lane] = M::finalize(w.cand_d[lane], qc, n0);
@@ -420,6 +421,111 @@ __device__ __forceinline__ void measure_list(device_index_t const& ix, search_ar
         for (uint32_t c = 64 + lane; c < ncand; c += 32) w.cand_d[c] = M::finalize(w.cand_d[c], qc, __ldg(ix.norms + w.cand_s[c]));
         __syncwarp();
     }
+}
+
+/*
+ *  The layer-0 list of a hop that starts with `top` full (cos / ip f32 with a shadow). The reference drops a candidate
+ *  with d >= radius without a trace: it is neither pushed nor inserted, and only `computed_distances` counts it. The
+ *  radius only shrinks inside a hop, so a candidate whose lower bound (prefilter_bound.h) reaches the radius at the start
+ *  of the hop is rejected at its turn too. Such candidates get +inf and never touch their f32 row; the others are
+ *  measured exactly and the accept replay that follows is unchanged. Returns the number of survivors.
+ *
+ *    1. TMA bulk copies put the int8 codes of up to `code_pass` candidates into the stage area, records load meanwhile;
+ *    2. 4 lanes per code form a.c in f32: lane `sub` of group g reads code word sub + 4 (t ^ g), so that the 8 groups hit
+ *       distinct banks although the codes sit 128-byte aligned (the order of the sum does not matter to the bound);
+ *    3. one lane per candidate evaluates the bound; a ballot lists the survivors in stored order;
+ *    4. the survivors' rows go through the STAGED pipeline, then their distances land in `cand_d` at their places.
+ */
+__device__ __forceinline__ pf_record_t ldg_record(pf_record_t const* p) {
+    float4 const v = __ldg(reinterpret_cast<float4 const*>(p));
+    return pf_record_t{v.x, v.y, v.z, v.w};
+}
+
+template <class M>
+__device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix, search_args_t const& a, warp_ctx_t& w,
+                                                     typename M::qconst_t qc, float a2, float radius, uint32_t ncand, int lane) {
+    uint8_t* const smem = reinterpret_cast<uint8_t*>(w.q4); /* the query opens the warp's shared memory */
+    uint32_t* const surv_s = reinterpret_cast<uint32_t*>(smem + a.off_surv_s); /* survivors: slots, places, values */
+    uint32_t* const surv_i = reinterpret_cast<uint32_t*>(smem + a.off_surv_i);
+    float* const surv_d = reinterpret_cast<float*>(smem + a.off_surv_d);
+    uint32_t const cs = ix.code_stride, scs = a.code_smem_stride, words = ix.chunks16;
+    uint32_t const tpad = ((words + 3) / 4 + 7) & ~7u; /* steps per lane, a multiple of 8 so that t ^ g stays inside */
+    uint32_t const bar = w.bars_addr;                  /* set 0's barrier */
+    uint32_t const g = (uint32_t)lane >> 2, sub = (uint32_t)lane & 3;
+    float4 const* const q4 = reinterpret_cast<float4 const*>(w.q4);
+    uint32_t ns = 0;
+    for (uint32_t base = 0; base < ncand; base += a.code_pass) {
+        uint32_t const cnt = min(a.code_pass, ncand - base); /* code_pass <= 64 */
+        if (lane == 0) mbar_expect_tx(bar, cnt * cs);
+        __syncwarp();
+        pf_record_t r0{}, r1{};
+        uint32_t const c0 = base + lane, c1 = base + lane + 32;
+        if ((uint32_t)lane < cnt) {
+            uint32_t const s = w.cand_s[c0];
+            bulk_copy_g2s(w.stage_addr + lane * scs, ix.codes + (size_t)s * cs, cs, bar);
+            r0 = ldg_record(ix.shadow + s);
+        }
+        if ((uint32_t)lane + 32 < cnt) {
+            uint32_t const s = w.cand_s[c1];
+            bulk_copy_g2s(w.stage_addr + (lane + 32) * scs, ix.codes + (size_t)s * cs, cs, bar);
+            r1 = ldg_record(ix.shadow + s);
+        }
+        mbar_wait(bar, w.phase & 1u);
+        w.phase ^= 1u;
+        for (uint32_t i0 = 0; i0 < cnt; i0 += 8) {
+            uint32_t const i = i0 + g;
+            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            if (i < cnt) {
+                uint32_t const* code = reinterpret_cast<uint32_t const*>(w.stage + (size_t)i * scs);
+#pragma unroll 4
+                for (uint32_t t = 0; t < tpad; ++t) {
+                    uint32_t const u = sub + 4u * (t ^ g);
+                    if (u < words) {
+                        uint32_t const cw = code[u] ^ 0x80808080u; /* biased bytes: 2^23 + (c + 128) as f32 bits, exact */
+                        float4 const q = q4[u];
+                        acc[0] = __fmaf_rn(q.x, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7540u)), 8388736.f), acc[0]);
+                        acc[1] = __fmaf_rn(q.y, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7541u)), 8388736.f), acc[1]);
+                        acc[2] = __fmaf_rn(q.z, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7542u)), 8388736.f), acc[2]);
+                        acc[3] = __fmaf_rn(q.w, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7543u)), 8388736.f), acc[3]);
+                    }
+                }
+            }
+            float dot = __fadd_rn(__fadd_rn(acc[0], acc[1]), __fadd_rn(acc[2], acc[3]));
+            dot = __fadd_rn(dot, __shfl_xor_sync(0xffffffffu, dot, 1));
+            dot = __fadd_rn(dot, __shfl_xor_sync(0xffffffffu, dot, 2));
+            if (i < cnt && sub == 0) w.cand_d[base + i] = dot;
+        }
+        __syncwarp(); /* dots visible, and every lane is done with the stage area before it is refilled */
+        uint32_t const lt = (1u << lane) - 1u;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            uint32_t const i = (uint32_t)lane + 32u * (uint32_t)h, c = base + i;
+            if (32u * (uint32_t)h >= cnt) break; /* uniform */
+            pf_record_t const r = h ? r1 : r0;
+            bool keep = false;
+            if (i < cnt) keep = !(M::pf_lower(w.cand_d[c], r, a2, ix.dims) >= (double)radius);
+            uint32_t const bal = __ballot_sync(0xffffffffu, keep);
+            if (keep) {
+                surv_s[ns + __popc(bal & lt)] = w.cand_s[c];
+                surv_i[ns + __popc(bal & lt)] = c;
+            }
+            if (i < cnt) w.cand_d[c] = keep ? r.b2 : __int_as_float(0x7f800000); /* survivors: the norm finalize needs */
+            ns += __popc(bal);
+        }
+        __syncwarp();
+    }
+    if (ns) {
+        measure_staged<M>(ix, a, w, qc, ns, lane, surv_s, surv_d);
+        __syncwarp();
+        for (uint32_t j = lane; j < ns; j += 32) {
+            uint32_t const c = surv_i[j];
+            float const raw = surv_d[j];
+            if constexpr (M::NORMS) w.cand_d[c] = M::finalize(raw, qc, w.cand_d[c]);
+            else w.cand_d[c] = raw;
+        }
+        __syncwarp();
+    }
+    return ns;
 }
 
 /* The predicate of index_dense_gt::search_ (index_dense.hpp:2071-2083): not the free key, and — for a
@@ -450,7 +556,9 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
     uint32_t visited_total = 0;
     bool log_overflow_out = false;
     bool const prof = a.phase_cycles != nullptr;
-    uint32_t pc0 = 0, pc1 = 0, pc2 = 0, pc4 = 0, pc5 = 0, n_push = 0, max_heap = 0;
+    uint32_t pc0 = 0, pc1 = 0, pc2 = 0, pc4 = 0, pc5 = 0, n_push = 0, max_heap = 0, n_pref = 0, n_surv = 0;
+    /* the layer-0 prefilter: plain searches of the f32 metrics that declare it, on an index that has the shadow */
+    constexpr bool PF = prefilter_of<M>::value && STAGED && !INSERT;
     long long tp = prof ? clock64() : 0;
     w.t_wait = 0;
 #define PHASE(acc)                                  \
@@ -497,6 +605,8 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         __threadfence_block();
         __syncwarp();
         typename M::qconst_t qc = M::prepare(w.q4, ix.chunks16, lane);
+        float pf_a2 = 0.f; /* the query's squared norm, as the reference accumulates it */
+        if constexpr (PF) pf_a2 = cos_f32_t::self_dot(w.q4, ix.chunks16, lane);
         uint32_t const vmask = a.visited_cap - 1;
         uint32_t visited_count = 0;
 
@@ -707,7 +817,16 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
             PHASE(pc2)
             if (ncand == 0) continue;
 
-            measure_list<M, STAGED>(ix, a, w, qc, ncand, lane);
+            bool measured = false;
+            if constexpr (PF) {
+                if (a.prefilter && top_size == ef) { /* `top` full: every candidate must beat the radius */
+                    uint32_t const ns = measure_prefiltered<M>(ix, a, w, qc, pf_a2, radius, ncand, lane);
+                    n_pref += ncand;
+                    n_surv += ns;
+                    measured = true;
+                }
+            }
+            if (!measured) measure_list<M, STAGED>(ix, a, w, qc, ncand, lane);
             computed += ncand;
             PHASE(pc4)
 
@@ -827,6 +946,8 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         atomicAdd(a.phase_cycles + 8, (unsigned long long)n_push);
         atomicAdd(a.phase_cycles + 9, (unsigned long long)max_heap);
         atomicMax(a.phase_cycles + 10, (unsigned long long)max_heap);
+        atomicAdd(a.phase_cycles + 11, (unsigned long long)n_pref);
+        atomicAdd(a.phase_cycles + 12, (unsigned long long)n_surv);
     }
 #undef PHASE
 }
@@ -943,6 +1064,65 @@ cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStr
         norms_kernel<cos_half_t<bf16_conv_t>><<<(ix.n + threads - 1) / threads, threads, 0, stream>>>(ix, norms);
     } else
         return cudaErrorInvalidValue;
+    return cudaGetLastError();
+}
+
+/* ---- the int8 shadow of cos / ip f32 rows (prefilter_bound.h): one warp per row -------------------------- */
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__global__ void shadow_kernel(device_index_t ix, float const* norms, int8_t* codes, pf_record_t* records) {
+    uint32_t const lane = threadIdx.x & 31, row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (row >= ix.n) return; /* uniform per warp */
+    float const* b = reinterpret_cast<float const*>(ix.vectors + (size_t)row * ix.vec_stride);
+    double mx = 0.0;
+    bool finite = true;
+    for (uint32_t i = lane; i < ix.dims; i += 32) {
+        double const x = fabs((double)b[i]);
+        finite = finite && x < INFINITY;
+        mx = fmax(mx, x);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    finite = __all_sync(0xffffffffu, finite);
+    float const s = pf_scale(mx);
+    bool const usable = finite && s > 0.0f;
+    double e2 = 0.0, n2 = 0.0;
+    int8_t* const c = codes + (size_t)row * ix.code_stride;
+    for (uint32_t i = lane; i < ix.code_stride; i += 32) {
+        int8_t q = 0;
+        if (usable && i < ix.dims) {
+            q = pf_code(b[i], s);
+            double const e = (double)b[i] - (double)s * (double)q;
+            e2 += e * e;
+            n2 += (double)b[i] * (double)b[i];
+        }
+        c[i] = q;
+    }
+    e2 = warp_sum_f64(e2);
+    n2 = warp_sum_f64(n2);
+    if (lane == 0) {
+        float const b2 = norms ? norms[row] : 0.f;
+        records[row] = usable ? pf_record_t{s, pf_round_up_norm(e2), pf_round_up_norm(n2), b2}
+                              : pf_record_t{0.f, INFINITY, INFINITY, b2};
+    }
+}
+
+bool search_is_staged(device_index_t const& ix);
+bool search_needs_shadow(device_index_t const& ix) {
+    return ix.scalar == SCALAR_F32 && (ix.metric == METRIC_COS || ix.metric == METRIC_IP) && search_is_staged(ix);
+}
+uint32_t search_code_stride(device_index_t const& ix) { return (ix.dims + 15u) & ~15u; }
+
+cudaError_t search_compute_shadow(device_index_t const& ix, float const* norms, int8_t* codes, pf_record_t* records,
+                                  cudaStream_t stream) {
+    if (!ix.n) return cudaSuccess;
+    uint32_t const rows_per_block = 8;
+    shadow_kernel<<<(ix.n + rows_per_block - 1) / rows_per_block, 32 * rows_per_block, 0, stream>>>(ix, norms, codes, records);
     return cudaGetLastError();
 }
 

@@ -501,7 +501,7 @@ class Index:
         return BatchMatches(keys, distances, counts, vm, cd)
 
     def tune(self, **knobs: int) -> None:
-        """Launch tuning knobs of this handle (stage_sets, warps_per_sm); results never change."""
+        """Launch tuning knobs of this handle (stage_sets, warps_per_sm, prefilter); results never change."""
         for name, value in knobs.items():
             if self._lib.usearch_b200_tune(self._h, name.encode(), int(value)) != 0:
                 raise ValueError(f"unknown knob {name}")
@@ -513,7 +513,8 @@ class Index:
         names = ["setup_descent", "heap_pop", "row_visited", "vector_wait", "distance_math", "accept", "output"]
         q = max(int(out[7]), 1)
         return {"queries": int(out[7]), **{n: float(out[i]) / q for i, n in enumerate(names)},
-                "pushes": float(out[8]) / q, "avg_max_heap": float(out[9]) / q, "max_heap": int(out[10])}
+                "pushes": float(out[8]) / q, "avg_max_heap": float(out[9]) / q, "max_heap": int(out[10]),
+                "prefiltered": float(out[11]) / q, "survivors": float(out[12]) / q}
 
     # ---- sharded search: this index is one shard of a group of processes (shards.cu) ------------------------
     def join_shards(self, rank: int, world: int, unique_id: bytes) -> None:
