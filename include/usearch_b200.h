@@ -255,7 +255,8 @@ size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries
  * counters summed over all queries since; `counters16` (may be NULL) first receives the current values:
  * cycles of setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay |
  * output, then queries | heap pushes | sum of per-query max heap size | max heap size | candidates prefiltered (layer-0
- * candidates of cos / ip f32 judged on their int8 shadow) | survivors (those of them whose f32 row was read) | 3 reserved. */
+ * candidates of cos / ip f32 judged on their int8 shadow) | survivors (those of them whose f32 row was read) | cycles
+ * of code wait (the prefilter waiting for its int8 codes; not part of distance math) | 2 reserved. */
 void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16);
 /* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
  * candidates of cos / ip f32 on their int8 shadow first, on by default); results never depend on them. Returns 0, or -1

@@ -119,9 +119,12 @@ struct search_args_t {
     uint32_t off_bars = 0, off_stage = 0, stage_stride = 0;
     uint32_t stage_sets = 1; /* 2 = double buffered: 2 x (32/LPV) slots, the next pass lands during the math */
     /* layer-0 prefilter (cos / ip f32 with a shadow): once `top` is full, a hop first bulk-copies the int8 codes of its
-     * candidates into the stage area (`code_pass` per pass, `code_smem_stride` bytes apart), rejects those whose lower
-     * bound proves d >= radius, and measures only the survivors (listed in surv_s / surv_i, exact values in surv_d) */
-    uint32_t prefilter = 0, code_pass = 0, code_smem_stride = 0, off_surv_s = 0, off_surv_i = 0, off_surv_d = 0;
+     * candidates into the stage area (`code_pass` per pass, `code_smem_stride` bytes apart), multiplies them on the
+     * tensor cores with the query's int8 split (off_qsplit: q1 then q2, `qsplit_len` bytes each), rejects those whose
+     * lower bound proves d >= radius, and measures only the survivors, compacted in `cand_s` (cos: their stored
+     * squared norms in surv_b2) */
+    uint32_t prefilter = 0, code_pass = 0, code_smem_stride = 0, off_surv_b2 = 0;
+    uint32_t off_qsplit = 0, qsplit_len = 0;
     /* optional introspection: 8 cycle counters summed over all queries (lane 0 clock64 deltas):
      * setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay | output, then counts
      * (include/usearch_b200.h, usearch_b200_profile_phases) */

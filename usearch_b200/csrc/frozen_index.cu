@@ -439,10 +439,11 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     pl.off_top_s = off; off += top_smem;
     pl.off_cand_s = off; off += list_cap * 4;
     pl.off_cand_d = off; off += list_cap * 4;
-    if (d.codes) { /* prefilter: the survivors of a list */
-        pl.off_surv_s = off; off += list_cap * 4;
-        pl.off_surv_i = off; off += list_cap * 4;
-        pl.off_surv_d = off; off += list_cap * 4;
+    /* prefilter: the tensor-core k-steps read 32 code bytes at a time, so the query split is zero-padded to that */
+    pl.qsplit_len = d.codes ? round_up(d.code_stride, 32) : 0;
+    if (d.codes) { /* prefilter: the survivors' stored squared norms, and the query split q1 | q2 */
+        pl.off_surv_b2 = off; off += list_cap * 4;
+        pl.off_qsplit = off; off += 2 * pl.qsplit_len;
     }
     pl.off_bars = off; off += 256; /* 32 mbarriers */
     off = round_up(off, 128);
@@ -470,9 +471,12 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     uint32_t const stage_bytes = (uint32_t)slots * pl.stage_sets * pl.stage_stride;
     off += stage_bytes;
     pl.off_heap = off;
-    /* prefilter: the int8 codes of a pass fill the stage area, 128-byte aligned, in whole groups of 8 (<= 64) */
-    pl.code_smem_stride = d.codes ? round_up(d.code_stride, 128) : 0;
-    pl.code_pass = d.codes ? std::min<uint32_t>(64, stage_bytes / pl.code_smem_stride) & ~7u : 0;
+    /* prefilter: the int8 codes of a pass fill the stage area in whole m16n8k32 tiles of 16 rows (<= 64). A row stride
+     * that is an odd multiple of 16 bytes puts the 8 rows of every ldmatrix matrix in distinct bank groups. The s32 dot
+     * products are exact while dims 127^2 < 2^31: above that the prefilter is off. */
+    pl.code_smem_stride = d.codes ? pl.qsplit_len + 16 : 0;
+    bool const s32_exact = (uint64_t)d.dims * 127u * 127u < (1ull << 31);
+    pl.code_pass = d.codes && s32_exact ? std::min<uint32_t>(64, stage_bytes / pl.code_smem_stride) & ~15u : 0;
     uint32_t const fixed = off;
     if (fixed + min_heap > smem_cta_max) return "Expansion or dimensionality too large for on-chip state";
     int const forced_warps = tune.warps_per_sm;
@@ -565,10 +569,11 @@ char const* frozen_index_t::prepare_launch(launch_plan_t const& pl, size_t warps
     a.off_cand_d = pl.off_cand_d; a.off_heap = pl.off_heap;
     a.off_bars = pl.off_bars; a.off_stage = pl.off_stage; a.stage_stride = pl.stage_stride;
     a.stage_sets = pl.stage_sets;
-    a.prefilter = tune.prefilter != 0 && pl.code_pass >= 8 ? 1u : 0u;
+    a.prefilter = tune.prefilter != 0 && pl.code_pass >= 16 ? 1u : 0u;
     a.code_pass = pl.code_pass;
     a.code_smem_stride = pl.code_smem_stride;
-    a.off_surv_s = pl.off_surv_s; a.off_surv_i = pl.off_surv_i; a.off_surv_d = pl.off_surv_d;
+    a.off_surv_b2 = pl.off_surv_b2;
+    a.off_qsplit = pl.off_qsplit; a.qsplit_len = pl.qsplit_len;
     return nullptr;
 }
 

@@ -53,7 +53,8 @@ struct launch_plan_t {
     size_t visited_words_per_warp() const { return visited_bitmap_words ? visited_bitmap_words : visited_cap; }
     uint32_t smem_per_warp = 0, off_top_d = 0, off_top_s = 0, off_cand_s = 0, off_cand_d = 0, off_heap = 0;
     uint32_t off_bars = 0, off_stage = 0, stage_stride = 0, stage_sets = 1;
-    uint32_t off_surv_s = 0, off_surv_i = 0, off_surv_d = 0, code_pass = 0, code_smem_stride = 0; /* prefilter */
+    uint32_t off_surv_b2 = 0, code_pass = 0, code_smem_stride = 0; /* prefilter */
+    uint32_t off_qsplit = 0, qsplit_len = 0;
     int blocks = 0;
     uint32_t warps_per_sm_target = 0;
     size_t smem_per_block = 0;

@@ -238,6 +238,7 @@ struct warp_ctx_t {
     uint32_t bars_addr;  /* shared-window address of the VPP mbarriers */
     uint32_t phase;      /* one parity bit per slot, uniform across the warp */
     uint32_t t_wait;     /* introspection: cycles spent waiting for staged vectors */
+    uint32_t t_code;     /* introspection: cycles spent waiting for the prefilter's int8 codes */
 };
 
 /* ---- distances of a whole candidate list ---------------------------------------------------- */
@@ -427,73 +428,157 @@ __device__ __forceinline__ void measure_list(device_index_t const& ix, search_ar
  *  The layer-0 list of a hop that starts with `top` full (cos / ip f32 with a shadow). The reference drops a candidate
  *  with d >= radius without a trace: it is neither pushed nor inserted, and only `computed_distances` counts it. The
  *  radius only shrinks inside a hop, so a candidate whose lower bound (prefilter_bound.h) reaches the radius at the start
- *  of the hop is rejected at its turn too. Such candidates get +inf and never touch their f32 row; the others are
- *  measured exactly and the accept replay that follows is unchanged. Returns the number of survivors.
+ *  of the hop is rejected at its turn too, and the accept replay never looks at it. So the survivors are compacted to
+ *  the front of the list in stored order, measured exactly, and the replay that follows visits only them. Rejected
+ *  candidates never touch their f32 row. Returns the number of survivors.
  *
  *    1. TMA bulk copies put the int8 codes of up to `code_pass` candidates into the stage area, records load meanwhile;
- *    2. 4 lanes per code form a.c in f32: lane `sub` of group g reads code word sub + 4 (t ^ g), so that the 8 groups hit
- *       distinct banks although the codes sit 128-byte aligned (the order of the sum does not matter to the bound);
+ *    2. the tensor cores form the exact integers D1 = q1.c and D2 = q2.c against the query's int8 split (split_query):
+ *       mma.sync m16n8k32 s8, the codes of 16 candidates as A (one ldmatrix.x4 per 32-byte k-step), q1 and q2 as
+ *       columns 0 and 1 of B (the other 6 are zero), s32 accumulators; `dot` = fl32(sa1 D1 + sa2 D2);
  *    3. one lane per candidate evaluates the bound; a ballot lists the survivors in stored order;
- *    4. the survivors' rows go through the STAGED pipeline, then their distances land in `cand_d` at their places.
+ *    4. the survivors' rows go through the STAGED pipeline, their distances land in `cand_d[0, ns)`.
  */
 __device__ __forceinline__ pf_record_t ldg_record(pf_record_t const* p) {
     float4 const v = __ldg(reinterpret_cast<float4 const*>(p));
     return pf_record_t{v.x, v.y, v.z, v.w};
 }
 
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__device__ __forceinline__ double warp_max_f64(double v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+/* The B fragment of m16n8k32 s8 gives lane `sub` of column g the k-bytes 4 sub .. 4 sub + 3 and 16 + 4 sub .. 16 + 4 sub
+ * + 3 of each 32-byte k-step. The split is stored with the words of a step in the order 0 4 1 5 2 6 3 7, so that one
+ * 8-byte load fetches both. */
+__device__ __forceinline__ uint32_t qsplit_word_place(uint32_t word) { return (word & ~7u) + (word & 3u) * 2u + ((word >> 2) & 1u); }
+
+/* pf_split_query (prefilter_bound.h) by one warp: the same element steps, the maxima and the sum of squares across lanes.
+ * `q1` and `q2` get `len` bytes each (zero beyond `n`) in the B-fragment order above. Uniform across the warp. */
+__device__ __forceinline__ pf_query_split_t split_query(float const* qa, uint32_t n, uint8_t* q1, uint8_t* q2, uint32_t len,
+                                                        int lane) {
+    double mx1 = 0.0;
+    bool finite = true;
+    for (uint32_t i = (uint32_t)lane; i < n; i += 32) {
+        double const x = fabs((double)qa[i]);
+        finite = finite && x < INFINITY;
+        mx1 = fmax(mx1, x);
+    }
+    mx1 = warp_max_f64(mx1);
+    finite = __all_sync(0xffffffffu, finite);
+    float const sa1 = pf_scale(mx1);
+    bool const usable = finite && sa1 > 0.0f;
+    double mx2 = 0.0;
+    int8_t c1, c2;
+    if (usable)
+        for (uint32_t i = (uint32_t)lane; i < n; i += 32) mx2 = fmax(mx2, fabs(pf_split_step((double)qa[i], sa1, c1)));
+    mx2 = warp_max_f64(mx2);
+    float const sa2 = usable ? pf_scale(mx2) : 0.0f;
+    double e2 = 0.0;
+    for (uint32_t wd = (uint32_t)lane; wd < len / 4; wd += 32) {
+        uint32_t p1 = 0, p2 = 0;
+#pragma unroll
+        for (uint32_t b = 0; b < 4; ++b) {
+            uint32_t const i = 4 * wd + b;
+            c1 = c2 = 0;
+            if (usable && i < n) {
+                double const r2 = pf_split_step(pf_split_step((double)qa[i], sa1, c1), sa2, c2);
+                e2 += r2 * r2;
+            }
+            p1 |= (uint32_t)(uint8_t)c1 << (8 * b);
+            p2 |= (uint32_t)(uint8_t)c2 << (8 * b);
+        }
+        reinterpret_cast<uint32_t*>(q1)[qsplit_word_place(wd)] = p1;
+        reinterpret_cast<uint32_t*>(q2)[qsplit_word_place(wd)] = p2;
+    }
+    e2 = warp_sum_f64(e2);
+    __syncwarp();
+    return usable ? pf_query_split_t{sa1, sa2, pf_round_up_norm(e2)} : pf_query_split_t{0.0f, 0.0f, INFINITY};
+}
+
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+                 : "r"(addr));
+}
+
+__device__ __forceinline__ void imma_16832(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
 template <class M>
 __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix, search_args_t const& a, warp_ctx_t& w,
-                                                     typename M::qconst_t qc, float a2, float radius, uint32_t ncand, int lane) {
+                                                     typename M::qconst_t qc, float a2, pf_query_split_t const& sp,
+                                                     float radius, uint32_t ncand, int lane) {
+    constexpr uint32_t MAX_TILES = 4; /* code_pass <= 64 */
     uint8_t* const smem = reinterpret_cast<uint8_t*>(w.q4); /* the query opens the warp's shared memory */
-    uint32_t* const surv_s = reinterpret_cast<uint32_t*>(smem + a.off_surv_s); /* survivors: slots, places, values */
-    uint32_t* const surv_i = reinterpret_cast<uint32_t*>(smem + a.off_surv_i);
-    float* const surv_d = reinterpret_cast<float*>(smem + a.off_surv_d);
-    uint32_t const cs = ix.code_stride, scs = a.code_smem_stride, words = ix.chunks16;
-    uint32_t const tpad = ((words + 3) / 4 + 7) & ~7u; /* steps per lane, a multiple of 8 so that t ^ g stays inside */
-    uint32_t const bar = w.bars_addr;                  /* set 0's barrier */
+    float* const surv_b2 = reinterpret_cast<float*>(smem + a.off_surv_b2); /* cos: the survivors' stored squared norms */
+    uint32_t const cs = ix.code_stride, scs = a.code_smem_stride, ksteps = a.qsplit_len / 32;
+    uint32_t const bar = w.bars_addr; /* set 0's barrier */
     uint32_t const g = (uint32_t)lane >> 2, sub = (uint32_t)lane & 3;
-    float4 const* const q4 = reinterpret_cast<float4 const*>(w.q4);
+    /* B: lanes 0-3 hold column 0 (q1), lanes 4-7 column 1 (q2); the other lanes' columns are zero */
+    uint32_t const b_addr = smem_u32(smem + a.off_qsplit) + g * a.qsplit_len + 8u * sub;
+    /* A: lane l gives the address of row l & 7 of matrix l >> 3: rows 0-7 / 8-15 of the tile, k-bytes 0-15 / 16-31 */
+    uint32_t const a_addr = w.stage_addr + ((uint32_t)lane & 7u) * scs + (((uint32_t)lane >> 3) & 1u) * 8u * scs + ((uint32_t)lane >> 4) * 16u;
+    double const sa1 = (double)sp.sa1, sa2 = (double)sp.sa2;
     uint32_t ns = 0;
     for (uint32_t base = 0; base < ncand; base += a.code_pass) {
         uint32_t const cnt = min(a.code_pass, ncand - base); /* code_pass <= 64 */
         if (lane == 0) mbar_expect_tx(bar, cnt * cs);
         __syncwarp();
         pf_record_t r0{}, r1{};
-        uint32_t const c0 = base + lane, c1 = base + lane + 32;
+        uint32_t s0 = 0, s1 = 0; /* slots of candidates base + lane and base + lane + 32 */
         if ((uint32_t)lane < cnt) {
-            uint32_t const s = w.cand_s[c0];
-            bulk_copy_g2s(w.stage_addr + lane * scs, ix.codes + (size_t)s * cs, cs, bar);
-            r0 = ldg_record(ix.shadow + s);
+            s0 = w.cand_s[base + lane];
+            bulk_copy_g2s(w.stage_addr + lane * scs, ix.codes + (size_t)s0 * cs, cs, bar);
+            r0 = ldg_record(ix.shadow + s0);
         }
         if ((uint32_t)lane + 32 < cnt) {
-            uint32_t const s = w.cand_s[c1];
-            bulk_copy_g2s(w.stage_addr + (lane + 32) * scs, ix.codes + (size_t)s * cs, cs, bar);
-            r1 = ldg_record(ix.shadow + s);
+            s1 = w.cand_s[base + lane + 32];
+            bulk_copy_g2s(w.stage_addr + (lane + 32) * scs, ix.codes + (size_t)s1 * cs, cs, bar);
+            r1 = ldg_record(ix.shadow + s1);
         }
-        mbar_wait(bar, w.phase & 1u);
+        if (a.phase_cycles) { /* introspection only: the wait for the codes goes to `code_wait` */
+            long long const t = clock64();
+            mbar_wait(bar, w.phase & 1u);
+            w.t_code += (uint32_t)(clock64() - t);
+        } else
+            mbar_wait(bar, w.phase & 1u);
         w.phase ^= 1u;
-        for (uint32_t i0 = 0; i0 < cnt; i0 += 8) {
-            uint32_t const i = i0 + g;
-            float acc[4] = {0.f, 0.f, 0.f, 0.f};
-            if (i < cnt) {
-                uint32_t const* code = reinterpret_cast<uint32_t const*>(w.stage + (size_t)i * scs);
-#pragma unroll 4
-                for (uint32_t t = 0; t < tpad; ++t) {
-                    uint32_t const u = sub + 4u * (t ^ g);
-                    if (u < words) {
-                        uint32_t const cw = code[u] ^ 0x80808080u; /* biased bytes: 2^23 + (c + 128) as f32 bits, exact */
-                        float4 const q = q4[u];
-                        acc[0] = __fmaf_rn(q.x, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7540u)), 8388736.f), acc[0]);
-                        acc[1] = __fmaf_rn(q.y, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7541u)), 8388736.f), acc[1]);
-                        acc[2] = __fmaf_rn(q.z, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7542u)), 8388736.f), acc[2]);
-                        acc[3] = __fmaf_rn(q.w, __fsub_rn(__uint_as_float(__byte_perm(cw, 0x4B000000u, 0x7543u)), 8388736.f), acc[3]);
-                    }
+        /* k outer, tiles inner: one B load per k-step serves every tile. Rows of the last tile beyond `cnt` hold stale
+         * bytes, and the k-bytes beyond `code_stride` of a row were never copied: the split is zero there, so they add 0
+         * to D1 and D2, and the rows' results are dropped. */
+        uint32_t const ntiles = (cnt + 15) / 16;
+        int acc[MAX_TILES][4] = {};
+#pragma unroll 2
+        for (uint32_t k = 0; k < ksteps; ++k) {
+            uint32_t b0 = 0, b1 = 0;
+            if (lane < 8) asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(b0), "=r"(b1) : "r"(b_addr + 32u * k));
+#pragma unroll
+            for (uint32_t t = 0; t < MAX_TILES; ++t) {
+                if (t < ntiles) { /* uniform */
+                    uint32_t a0, a1, a2r, a3;
+                    ldmatrix_x4(a_addr + t * 16u * scs + 32u * k, a0, a1, a2r, a3);
+                    imma_16832(acc[t], a0, a1, a2r, a3, b0, b1);
                 }
             }
-            float dot = __fadd_rn(__fadd_rn(acc[0], acc[1]), __fadd_rn(acc[2], acc[3]));
-            dot = __fadd_rn(dot, __shfl_xor_sync(0xffffffffu, dot, 1));
-            dot = __fadd_rn(dot, __shfl_xor_sync(0xffffffffu, dot, 2));
-            if (i < cnt && sub == 0) w.cand_d[base + i] = dot;
+        }
+        /* C: lane 4 g holds columns 0 and 1 (D1, D2) of rows g and g + 8 */
+#pragma unroll
+        for (uint32_t t = 0; t < MAX_TILES; ++t) {
+            uint32_t const i = 16u * t + g;
+            if (sub == 0 && i < cnt) w.cand_d[base + i] = __double2float_rn(sa1 * (double)acc[t][0] + sa2 * (double)acc[t][1]);
+            if (sub == 0 && i + 8 < cnt) w.cand_d[base + i + 8] = __double2float_rn(sa1 * (double)acc[t][2] + sa2 * (double)acc[t][3]);
         }
         __syncwarp(); /* dots visible, and every lane is done with the stage area before it is refilled */
         uint32_t const lt = (1u << lane) - 1u;
@@ -503,27 +588,23 @@ __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix
             if (32u * (uint32_t)h >= cnt) break; /* uniform */
             pf_record_t const r = h ? r1 : r0;
             bool keep = false;
-            if (i < cnt) keep = !(M::pf_lower(w.cand_d[c], r, a2, ix.dims) >= (double)radius);
+            if (i < cnt) keep = !(M::pf_lower(w.cand_d[c], r, a2, ix.dims, sp.rho_a) >= (double)radius);
             uint32_t const bal = __ballot_sync(0xffffffffu, keep);
-            if (keep) {
-                surv_s[ns + __popc(bal & lt)] = w.cand_s[c];
-                surv_i[ns + __popc(bal & lt)] = c;
+            if (keep) { /* in place: ns + rank <= c, and the slots of this pass are in registers */
+                w.cand_s[ns + __popc(bal & lt)] = h ? s1 : s0;
+                surv_b2[ns + __popc(bal & lt)] = r.b2;
             }
-            if (i < cnt) w.cand_d[c] = keep ? r.b2 : __int_as_float(0x7f800000); /* survivors: the norm finalize needs */
             ns += __popc(bal);
         }
         __syncwarp();
     }
     if (ns) {
-        measure_staged<M>(ix, a, w, qc, ns, lane, surv_s, surv_d);
+        measure_staged<M>(ix, a, w, qc, ns, lane, w.cand_s, w.cand_d);
         __syncwarp();
-        for (uint32_t j = lane; j < ns; j += 32) {
-            uint32_t const c = surv_i[j];
-            float const raw = surv_d[j];
-            if constexpr (M::NORMS) w.cand_d[c] = M::finalize(raw, qc, w.cand_d[c]);
-            else w.cand_d[c] = raw;
+        if constexpr (M::NORMS) {
+            for (uint32_t j = lane; j < ns; j += 32) w.cand_d[j] = M::finalize(w.cand_d[j], qc, surv_b2[j]);
+            __syncwarp();
         }
-        __syncwarp();
     }
     return ns;
 }
@@ -561,6 +642,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
     constexpr bool PF = prefilter_of<M>::value && STAGED && !INSERT;
     long long tp = prof ? clock64() : 0;
     w.t_wait = 0;
+    w.t_code = 0;
 #define PHASE(acc)                                  \
     if (prof) {                                     \
         long long now_ = clock64();                 \
@@ -606,7 +688,14 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         __syncwarp();
         typename M::qconst_t qc = M::prepare(w.q4, ix.chunks16, lane);
         float pf_a2 = 0.f; /* the query's squared norm, as the reference accumulates it */
-        if constexpr (PF) pf_a2 = cos_f32_t::self_dot(w.q4, ix.chunks16, lane);
+        pf_query_split_t pf_sp{0.f, 0.f, INFINITY}; /* the query's int8 split, the B operand of the prefilter */
+        if constexpr (PF) {
+            pf_a2 = cos_f32_t::self_dot(w.q4, ix.chunks16, lane);
+            if (a.prefilter) {
+                uint8_t* const q1 = reinterpret_cast<uint8_t*>(w.q4) + a.off_qsplit;
+                pf_sp = split_query(reinterpret_cast<float const*>(w.q4), ix.dims, q1, q1 + a.qsplit_len, a.qsplit_len, lane);
+            }
+        }
         uint32_t const vmask = a.visited_cap - 1;
         uint32_t visited_count = 0;
 
@@ -818,11 +907,12 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
             if (ncand == 0) continue;
 
             bool measured = false;
+            uint32_t nacc = ncand; /* the candidates the accept replay visits */
             if constexpr (PF) {
                 if (a.prefilter && top_size == ef) { /* `top` full: every candidate must beat the radius */
-                    uint32_t const ns = measure_prefiltered<M>(ix, a, w, qc, pf_a2, radius, ncand, lane);
+                    nacc = measure_prefiltered<M>(ix, a, w, qc, pf_a2, pf_sp, radius, ncand, lane);
                     n_pref += ncand;
-                    n_surv += ns;
+                    n_surv += nacc;
                     measured = true;
                 }
             }
@@ -833,9 +923,9 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
             /* The reference's sequential accept loop, replayed in stored order. `radius` only shrinks
              * and `top` only grows inside a hop, so a candidate that fails `|top|<ef || d<radius` at the
              * start of the hop fails it at its turn as well: only the others are visited. */
-            for (uint32_t b = 0; b < ncand && status == STATUS_OK; b += 32) {
+            for (uint32_t b = 0; b < nacc && status == STATUS_OK; b += 32) {
                 uint32_t c = b + lane;
-                bool maybe = c < ncand && (top_size < ef || cand_d[c] < radius);
+                bool maybe = c < nacc && (top_size < ef || cand_d[c] < radius);
                 uint32_t todo = __ballot_sync(0xffffffffu, maybe);
                 while (todo) {
                     uint32_t c2 = b + (__ffs(todo) - 1);
@@ -939,7 +1029,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         atomicAdd(a.phase_cycles + 1, (unsigned long long)pc1);
         atomicAdd(a.phase_cycles + 2, (unsigned long long)pc2);
         atomicAdd(a.phase_cycles + 3, (unsigned long long)w.t_wait);
-        atomicAdd(a.phase_cycles + 4, (unsigned long long)(pc4 - w.t_wait));
+        atomicAdd(a.phase_cycles + 4, (unsigned long long)(pc4 - w.t_wait - w.t_code));
         atomicAdd(a.phase_cycles + 5, (unsigned long long)pc5);
         atomicAdd(a.phase_cycles + 6, (unsigned long long)pc6);
         atomicAdd(a.phase_cycles + 7, 1ull);
@@ -948,6 +1038,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         atomicMax(a.phase_cycles + 10, (unsigned long long)max_heap);
         atomicAdd(a.phase_cycles + 11, (unsigned long long)n_pref);
         atomicAdd(a.phase_cycles + 12, (unsigned long long)n_surv);
+        atomicAdd(a.phase_cycles + 13, (unsigned long long)w.t_code);
     }
 #undef PHASE
 }
@@ -1068,12 +1159,6 @@ cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStr
 }
 
 /* ---- the int8 shadow of cos / ip f32 rows (prefilter_bound.h): one warp per row -------------------------- */
-
-__device__ __forceinline__ double warp_sum_f64(double v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 __global__ void shadow_kernel(device_index_t ix, float const* norms, int8_t* codes, pf_record_t* records) {
     uint32_t const lane = threadIdx.x & 31, row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;

@@ -514,7 +514,7 @@ class Index:
         q = max(int(out[7]), 1)
         return {"queries": int(out[7]), **{n: float(out[i]) / q for i, n in enumerate(names)},
                 "pushes": float(out[8]) / q, "avg_max_heap": float(out[9]) / q, "max_heap": int(out[10]),
-                "prefiltered": float(out[11]) / q, "survivors": float(out[12]) / q}
+                "prefiltered": float(out[11]) / q, "survivors": float(out[12]) / q, "code_wait": float(out[13]) / q}
 
     # ---- sharded search: this index is one shard of a group of processes (shards.cu) ------------------------
     def join_shards(self, rank: int, world: int, unique_id: bytes) -> None:
