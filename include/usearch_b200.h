@@ -259,9 +259,17 @@ size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries
  * of code wait (the prefilter waiting for its int8 codes; not part of distance math) | 2 reserved. */
 void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16);
 /* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
- * candidates of cos / ip f32 on their int8 shadow first, on by default); results never depend on them. Returns 0, or -1
- * for an unknown knob. */
+ * candidates of cos / ip f32 on their int8 shadow first, on by default; "heap_head" = an upper bound on the candidate-heap
+ * entries kept in shared memory, rounded down to an even number >= 2, the rest go to HBM; 0 = as planned); results never
+ * depend on them. Returns 0, or -1 for an unknown knob. */
 int usearch_b200_tune(usearch_index_t index, char const* knob, int value);
+/* The launch plan a search of `count` neighbours gets under the current knobs, for a loaded index. `out16` receives:
+ * stage sets | warps per SM (target) | blocks | shared memory per warp (bytes) | heap entries in shared memory | heap
+ * entries in HBM per warp | visits (0 = hash table, 1 = bitmap, 2 = bitmap cleaned through a log) | hash table entries |
+ * prefilter candidates per code pass | prefilter code row stride in shared memory (bytes) | bytes of each int8 query
+ * split level | prefilter effective (0 | 1) | stage area (bytes) | 3 reserved.
+ * Returns 0, or -1 with `error` set to the planner's message when no plan fits. */
+int usearch_b200_launch_plan(usearch_index_t index, size_t count, uint64_t* out16, usearch_error_t* error);
 int usearch_b200_device(usearch_index_t index);
 uint64_t usearch_b200_kernel_launches(usearch_index_t index);
 float usearch_b200_last_kernel_ms(usearch_index_t index);

@@ -69,6 +69,18 @@ def test_init_and_metadata_without_gpu():
         Index(ndim=64, metric="haversine", dtype="f32")
 
 
+def test_tune_knobs_and_launch_plan_of_an_empty_index():
+    """Every documented knob is accepted, an unknown one is refused, and an index without members has no plan to read."""
+    from usearch_b200.index import Index
+    index = Index(ndim=8, metric="cos", dtype="f32")
+    index.tune(stage_sets=2, warps_per_sm=1, prefilter=0, heap_head=2)
+    index.tune(stage_sets=0, warps_per_sm=0, prefilter=1, heap_head=0)
+    with pytest.raises(ValueError, match="unknown knob"):
+        index.tune(heap_tail=2)
+    with pytest.raises(RuntimeError, match="no CPU fallback|no launch plan"):
+        index.launch_plan(4)
+
+
 def test_load_fails_loudly_without_cuda_device():
     import torch
     if torch.cuda.is_available():

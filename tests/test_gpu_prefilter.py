@@ -89,13 +89,11 @@ def test_prefilter_after_add_many(metric):
     _check(index, _pinned(saved, q, k, ef), q, k, f"{metric} grown")
 
 
-@pytest.mark.parametrize("metric", ["cos", "ip"])
-def test_prefilter_near_duplicate_rows(metric):
-    """Clusters of rows one or a few ULPs apart (and exact duplicates): distances tie or differ in the last bits, where
-    only an exact bound keeps the reference's choices."""
-    from usearch_b200.index import Index
+def _near_duplicate_rows(d=256):
+    """300 clusters of 20 rows: each centre, a duplicate of it, and 18 copies with every element one ULP up or down; 256
+    queries close to random centres."""
     rng = np.random.default_rng(7)
-    centres, copies, d, m, ef, k = 300, 20, 256, 16, 64, 10
+    centres, copies = 300, 20
     c = rng.standard_normal((centres, d), dtype=np.float32)
     base = np.repeat(c, copies, axis=0)
     up = rng.integers(0, 2, size=base.shape).astype(bool)  # every element one ULP up or down
@@ -103,6 +101,16 @@ def test_prefilter_near_duplicate_rows(metric):
     base[::copies] = c  # one exact copy of each centre
     base[1::copies] = c  # and a duplicate of it
     q = (c[rng.integers(0, centres, 256)] + 1e-3 * rng.standard_normal((256, d), dtype=np.float32)).astype(np.float32)
+    return base, q
+
+
+@pytest.mark.parametrize("metric", ["cos", "ip"])
+def test_prefilter_near_duplicate_rows(metric):
+    """Clusters of rows one or a few ULPs apart (and exact duplicates): distances tie or differ in the last bits, where
+    only an exact bound keeps the reference's choices."""
+    from usearch_b200.index import Index
+    d, m, ef, k = 256, 16, 64, 10
+    base, q = _near_duplicate_rows(d)
     _, blob = common.build_reference_blob(base, metric, "f32", d, m, threads=16)
     index = Index.restore(blob)
     index.expansion_search = ef

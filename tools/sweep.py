@@ -3,7 +3,8 @@
     python tools/sweep.py --workload NS --configs "base;warps_per_sm=3;stage_sets=1" --steps 6
 
 Prints one JSON line per configuration: kernel ms per launch (CUDA events inside the library), algorithmic GB/s and the
-fraction of the measured HBM peak (the roofline figure of bench.py), recall on the first batch."""
+fraction of the measured HBM peak (the roofline figure of bench.py), recall on the first batch, and the launch plan the
+configuration got (Index.launch_plan)."""
 import argparse
 import json
 import os
@@ -62,7 +63,7 @@ def main():
     m0 = 2 * index.connectivity
     print(json.dumps({"workload": bench.workload_name(a), "build_s": round(build_s, 1), "hbm_gb": round(index.memory_usage / 1e9, 2)}), flush=True)
     for spec in o.configs.split(";"):
-        knobs = {"stage_sets": 0, "warps_per_sm": 0, "prefilter": 1}
+        knobs = {"stage_sets": 0, "warps_per_sm": 0, "prefilter": 1, "heap_head": 0}
         if spec != "base":
             for kv in spec.split(","):
                 name, value = kv.split("=")
@@ -89,7 +90,7 @@ def main():
         k_ms = float(np.mean(ms))
         gbs = float(np.mean(alg)) / (k_ms * 1e-3) / 1e9
         line = {"config": spec, "kernel_ms": round(k_ms, 3), "qps": round(B / (k_ms * 1e-3)), "alg_gbs": round(gbs, 1), "frac": round(gbs / peak, 4),
-                "recall_at_10": round(rec, 4)}
+                "recall_at_10": round(rec, 4), "plan": index.launch_plan(k)}
         if o.phases:
             ph = index.profile_phases(False)
             line["phases"] = {k2: round(v, 1) for k2, v in ph.items()}

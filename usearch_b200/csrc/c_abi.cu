@@ -568,7 +568,26 @@ int usearch_b200_tune(usearch_index_t index, char const* knob, int value) {
     if (!std::strcmp(knob, "stage_sets")) ix->tune.stage_sets = value;
     else if (!std::strcmp(knob, "warps_per_sm")) ix->tune.warps_per_sm = value;
     else if (!std::strcmp(knob, "prefilter")) ix->tune.prefilter = value;
+    else if (!std::strcmp(knob, "heap_head")) ix->tune.heap_head = value;
     else return -1;
+    return 0;
+}
+
+int usearch_b200_launch_plan(usearch_index_t index, size_t count, uint64_t* out16, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    char const* e = ix->ensure_context();
+    if (!e && (!ix->loaded || ix->d.n == 0)) e = "An empty index has no launch plan";
+    launch_plan_t pl;
+    if (!e) e = ix->plan((uint32_t)count, 0, pl);
+    set_error(error, e);
+    if (e) return -1;
+    uint64_t const visits = pl.visited_bitmap_words ? (pl.visit_log_cap ? 2u : 1u) : 0u;
+    uint64_t const v[16] = {pl.stage_sets, pl.warps_per_sm_target, (uint64_t)pl.blocks, pl.smem_per_warp,
+                            pl.heap_smem_cap, pl.heap_spill_cap, visits, pl.visited_cap,
+                            pl.code_pass, pl.code_smem_stride, pl.qsplit_len, pl.prefilter ? 1u : 0u,
+                            pl.off_heap - pl.off_stage};
+    std::memcpy(out16, v, sizeof(v));
     return 0;
 }
 

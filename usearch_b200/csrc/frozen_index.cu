@@ -431,53 +431,61 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     /* `visits` covers every slot the arrays have room for, so that its size does not change while members are added */
     uint64_t const visit_slots = std::max<uint64_t>(capacity, d.n);
     uint32_t const list_cap = round_up(std::max(d.m0, d.m), 32);
-    /* per-warp (= per-CTA) shared memory: query | top | candidates | mbarriers | TMA slots | heap head */
-    uint32_t off = 0;
-    off += d.chunks16 * 16;          /* query */
-    uint32_t const top_smem = ef > 256 ? round_up(ef * 4, 16) : 0; /* ef <= 256: `top` lives in registers */
-    pl.off_top_d = off; off += top_smem;
-    pl.off_top_s = off; off += top_smem;
-    pl.off_cand_s = off; off += list_cap * 4;
-    pl.off_cand_d = off; off += list_cap * 4;
-    /* prefilter: the tensor-core k-steps read 32 code bytes at a time, so the query split is zero-padded to that */
-    pl.qsplit_len = d.codes ? round_up(d.code_stride, 32) : 0;
-    if (d.codes) { /* prefilter: the survivors' stored squared norms, and the query split q1 | q2 */
-        pl.off_surv_b2 = off; off += list_cap * 4;
-        pl.off_qsplit = off; off += 2 * pl.qsplit_len;
-    }
-    pl.off_bars = off; off += 256; /* 32 mbarriers */
-    off = round_up(off, 128);
-    pl.off_stage = off;
-    int const slots = search_stage_slots(d); /* slots of one set: 32 / LPV */
     /* an SM has 228 KB of shared memory and charges 1 KB per resident CTA on top of its request */
     size_t const smem_sm = 228 * 1024, cta_tax = 1024, smem_cta_max = 227 * 1024;
     uint32_t const min_heap = 128 * 8;
-    int const forced_sets = tune.stage_sets;
-    pl.stage_sets = 1;
-    pl.stage_stride = 0;
-    if (slots) {
-        /* slot stride = 16*LPV mod 128 bytes: the lanes of a quarter-warp then read disjoint banks */
-        pl.stage_stride = round_up(d.chunks16 * 16, 128) + search_stage_pad(d);
-        /* double-buffer the slots when at least 4 warps per SM still fit */
-        size_t const two = off + 2 * (size_t)slots * pl.stage_stride + min_heap + cta_tax;
-        pl.stage_sets = smem_sm / two >= 4 ? 2u : 1u;
-        /* short vectors of the 16-warp kernels: resident warps beat double buffering (search_kernel.cu, dispatch) */
-        if (search_single_stage_set(d)) pl.stage_sets = 1;
-        /* prefilter on: a hop reads few rows, so resident warps beat double buffering (C2 on one H100 SXM at 700 W: 14.9 ms
-         * per 4096-query launch with one set and 7 warps per SM, 18.2 ms with two sets and 4) */
-        if (d.codes && tune.prefilter) pl.stage_sets = 1;
-        if (forced_sets == 1 || forced_sets == 2) pl.stage_sets = (uint32_t)forced_sets;
-    }
-    uint32_t const stage_bytes = (uint32_t)slots * pl.stage_sets * pl.stage_stride;
-    off += stage_bytes;
-    pl.off_heap = off;
-    /* prefilter: the int8 codes of a pass fill the stage area in whole m16n8k32 tiles of 16 rows (<= 64). A row stride
-     * that is an odd multiple of 16 bytes puts the 8 rows of every ldmatrix matrix in distinct bank groups. The s32 dot
-     * products are exact while dims 127^2 < 2^31: above that the prefilter is off. */
-    pl.code_smem_stride = d.codes ? pl.qsplit_len + 16 : 0;
+    /* The prefilter's s32 dot products are exact while dims 127^2 < 2^31: above that it is off. Only a plain search can
+     * run it (the builder's INSERT kernel never does), and its shared memory is reserved only then. Where that layout
+     * does not fit, the search goes without the prefilter rather than fail. */
     bool const s32_exact = (uint64_t)d.dims * 127u * 127u < (1ull << 31);
-    pl.code_pass = d.codes && s32_exact ? std::min<uint32_t>(64, stage_bytes / pl.code_smem_stride) & ~15u : 0;
-    uint32_t const fixed = off;
+    uint32_t fixed = 0;
+    for (bool pf = d.codes && tune.prefilter && s32_exact && !ef_override;; pf = false) {
+        /* per-warp (= per-CTA) shared memory: query | top | candidates | mbarriers | TMA slots | heap head */
+        uint32_t off = 0;
+        off += d.chunks16 * 16;          /* query */
+        uint32_t const top_smem = ef > 256 ? round_up(ef * 4, 16) : 0; /* ef <= 256: `top` lives in registers */
+        pl.off_top_d = off; off += top_smem;
+        pl.off_top_s = off; off += top_smem;
+        pl.off_cand_s = off; off += list_cap * 4;
+        pl.off_cand_d = off; off += list_cap * 4;
+        /* prefilter: the tensor-core k-steps read 32 code bytes at a time, so the query split is zero-padded to that */
+        pl.qsplit_len = pf ? round_up(d.code_stride, 32) : 0;
+        pl.off_surv_b2 = pl.off_qsplit = 0;
+        if (pf) { /* prefilter: the survivors' stored squared norms, and the query split q1 | q2 */
+            pl.off_surv_b2 = off; off += list_cap * 4;
+            pl.off_qsplit = off; off += 2 * pl.qsplit_len;
+        }
+        pl.off_bars = off; off += 256; /* 32 mbarriers */
+        off = round_up(off, 128);
+        pl.off_stage = off;
+        int const slots = search_stage_slots(d); /* slots of one set: 32 / LPV */
+        int const forced_sets = tune.stage_sets;
+        pl.stage_sets = 1;
+        pl.stage_stride = 0;
+        if (slots) {
+            /* slot stride = 16*LPV mod 128 bytes: the lanes of a quarter-warp then read disjoint banks */
+            pl.stage_stride = round_up(d.chunks16 * 16, 128) + search_stage_pad(d);
+            /* double-buffer the slots when at least 4 warps per SM still fit */
+            size_t const two = off + 2 * (size_t)slots * pl.stage_stride + min_heap + cta_tax;
+            pl.stage_sets = smem_sm / two >= 4 ? 2u : 1u;
+            /* short vectors of the 16-warp kernels: resident warps beat double buffering (search_kernel.cu, dispatch) */
+            if (search_single_stage_set(d)) pl.stage_sets = 1;
+            /* prefilter on: a hop reads few rows, so resident warps beat double buffering (C2 on one H100 SXM at 700 W: 14.9 ms
+             * per 4096-query launch with one set and 7 warps per SM, 18.2 ms with two sets and 4) */
+            if (d.codes && tune.prefilter) pl.stage_sets = 1;
+            if (forced_sets == 1 || forced_sets == 2) pl.stage_sets = (uint32_t)forced_sets;
+        }
+        uint32_t const stage_bytes = (uint32_t)slots * pl.stage_sets * pl.stage_stride;
+        off += stage_bytes;
+        pl.off_heap = off;
+        /* prefilter: the int8 codes of a pass fill the stage area in whole m16n8k32 tiles of 16 rows (<= 64). A row stride
+         * that is an odd multiple of 16 bytes puts the 8 rows of every ldmatrix matrix in distinct bank groups. */
+        pl.code_smem_stride = pf ? pl.qsplit_len + 16 : 0;
+        pl.code_pass = pf ? std::min<uint32_t>(64, stage_bytes / pl.code_smem_stride) & ~15u : 0;
+        pl.prefilter = pl.code_pass >= 16;
+        fixed = off;
+        if (!pf || fixed + min_heap <= smem_cta_max) break;
+    }
     if (fixed + min_heap > smem_cta_max) return "Expansion or dimensionality too large for on-chip state";
     int const forced_warps = tune.warps_per_sm;
     uint32_t warps_sm = (uint32_t)std::min<size_t>(smem_sm / (fixed + min_heap + cta_tax), (size_t)search_max_warps_per_sm(d));
@@ -486,6 +494,8 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     uint32_t budget = (uint32_t)(smem_sm / warps_sm - cta_tax);
     budget = std::min<uint32_t>(budget, (uint32_t)smem_cta_max);
     uint32_t heap_bytes = std::min<uint32_t>((budget - fixed) & ~15u, 4096 * 8);
+    /* the heap_head knob: a smaller head sends more of the heap to its HBM tail; the root stays in shared memory */
+    if (tune.heap_head > 0) heap_bytes = std::min<uint32_t>(heap_bytes, (uint32_t)std::max(tune.heap_head / 2, 1) * 16);
     pl.heap_smem_cap = heap_bytes / 8; /* even: heap_bytes is a multiple of 16 */
     pl.smem_per_warp = fixed + pl.heap_smem_cap * 8;
     pl.smem_per_block = pl.smem_per_warp;
@@ -569,7 +579,7 @@ char const* frozen_index_t::prepare_launch(launch_plan_t const& pl, size_t warps
     a.off_cand_d = pl.off_cand_d; a.off_heap = pl.off_heap;
     a.off_bars = pl.off_bars; a.off_stage = pl.off_stage; a.stage_stride = pl.stage_stride;
     a.stage_sets = pl.stage_sets;
-    a.prefilter = tune.prefilter != 0 && pl.code_pass >= 16 ? 1u : 0u;
+    a.prefilter = pl.prefilter ? 1u : 0u;
     a.code_pass = pl.code_pass;
     a.code_smem_stride = pl.code_smem_stride;
     a.off_surv_b2 = pl.off_surv_b2;

@@ -55,6 +55,7 @@ struct launch_plan_t {
     uint32_t off_bars = 0, off_stage = 0, stage_stride = 0, stage_sets = 1;
     uint32_t off_surv_b2 = 0, code_pass = 0, code_smem_stride = 0; /* prefilter */
     uint32_t off_qsplit = 0, qsplit_len = 0;
+    bool prefilter = false; /* the layout above has room for the prefilter and the knobs let it run */
     int blocks = 0;
     uint32_t warps_per_sm_target = 0;
     size_t smem_per_block = 0;
@@ -148,12 +149,14 @@ struct frozen_index_t {
     bool loaded = false;
     void* dev_allocs[10] = {nullptr}; /* vectors keys nbr0 upper_base upper deleted norms - codes shadow */
 
-    /* tuning knobs of the search launch: environment at construction (USEARCH_B200_STAGE_SETS, _WARPS_PER_SM),
-     * changeable per handle with usearch_b200_tune (bench sweeps, tests) */
+    /* tuning knobs of the search launch: environment at construction (USEARCH_B200_STAGE_SETS, _WARPS_PER_SM,
+     * _PREFILTER, _HEAP_HEAD), changeable per handle with usearch_b200_tune (bench sweeps, tests) */
     struct tune_t {
         int stage_sets = env_int("USEARCH_B200_STAGE_SETS", 0);     /* 0 = planned, 1 or 2 = forced */
         int warps_per_sm = env_int("USEARCH_B200_WARPS_PER_SM", 0); /* 0 = as many as fit, else an upper bound */
         int prefilter = env_int("USEARCH_B200_PREFILTER", 1);       /* 0 = measure every layer-0 candidate exactly */
+        int heap_head = env_int("USEARCH_B200_HEAP_HEAD", 0);       /* 0 = as planned, else an upper bound on the heap
+                                                                       entries kept in shared memory (even, >= 2) */
         static int env_int(char const* name, int fallback) {
             char const* v = std::getenv(name);
             return v ? std::atoi(v) : fallback;

@@ -54,7 +54,13 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_shards_unique_id", "usearch_b200_shards_join", "usearch_b200_sharded_search_many",
     "usearch_b200_sharded_search_many_device", "usearch_b200_shards_payload_bytes", "usearch_b200_merge_topk",
     "usearch_b200_search_many_enqueue", "usearch_b200_search_many_finish", "usearch_b200_tune",
+    "usearch_b200_launch_plan",
 ]
+
+# the fields of usearch_b200_launch_plan, in order
+LAUNCH_PLAN_FIELDS = ["stage_sets", "warps_per_sm_target", "blocks", "smem_per_warp", "heap_smem_cap", "heap_spill_cap",
+                      "visits", "visited_cap", "code_pass", "code_smem_stride", "qsplit_len", "prefilter", "stage_bytes"]
+_VISITS = ["hash", "bitmap", "bitmap_log"]
 
 
 def load_library() -> C.CDLL:
@@ -103,6 +109,8 @@ def load_library() -> C.CDLL:
     lib.usearch_b200_search_many_finish.argtypes = [C.c_void_p, err]
     lib.usearch_b200_tune.restype = C.c_int
     lib.usearch_b200_tune.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+    lib.usearch_b200_launch_plan.restype = C.c_int
+    lib.usearch_b200_launch_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, err]
     lib.usearch_b200_filtered_search_many.restype = C.c_size_t
     lib.usearch_b200_filtered_search_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int,
                                                       C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
@@ -501,10 +509,22 @@ class Index:
         return BatchMatches(keys, distances, counts, vm, cd)
 
     def tune(self, **knobs: int) -> None:
-        """Launch tuning knobs of this handle (stage_sets, warps_per_sm, prefilter); results never change."""
+        """Launch tuning knobs of this handle (stage_sets, warps_per_sm, prefilter, heap_head); results never change."""
         for name, value in knobs.items():
             if self._lib.usearch_b200_tune(self._h, name.encode(), int(value)) != 0:
                 raise ValueError(f"unknown knob {name}")
+
+    def launch_plan(self, count: int = 10) -> dict:
+        """The launch plan a search of `count` neighbours gets under the current knobs (see include/usearch_b200.h).
+        Raises the planner's error when no plan fits, as `search` would."""
+        out = np.zeros(16, dtype=np.uint64)
+        err = C.c_char_p()
+        self._lib.usearch_b200_launch_plan(self._h, int(count), out.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        plan = dict(zip(LAUNCH_PLAN_FIELDS, (int(v) for v in out)))
+        plan["visits"] = _VISITS[plan["visits"]]
+        plan["prefilter"] = bool(plan["prefilter"])
+        return plan
 
     def profile_phases(self, enable: bool = True) -> dict:
         """Read (then reset) the kernel's per-phase cycle counters; see include/usearch_b200.h."""
