@@ -256,7 +256,9 @@ size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries
  * cycles of setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay |
  * output, then queries | heap pushes | sum of per-query max heap size | max heap size | candidates prefiltered (layer-0
  * candidates of cos / ip f32 judged on their int8 shadow) | survivors (those of them whose f32 row was read) | cycles
- * of code wait (the prefilter waiting for its int8 codes; not part of distance math) | 2 reserved. */
+ * of code wait (the prefilter waiting for its int8 codes; not part of distance math) | cycles of the prefilter's dot
+ * products (the tensor-core dots and their conversion; part of distance math) | cycles of the prefilter's bound (the
+ * bound, its ballots and the survivors' compaction; part of distance math). */
 void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16);
 /* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
  * candidates of cos / ip f32 on their int8 shadow first, on by default; "heap_head" = an upper bound on the candidate-heap

@@ -97,6 +97,7 @@ def main():
             # bytes the kernel moved per query: the vectors it read, the codes and records of prefiltered candidates, the
             # lists of the hops (the algorithmic figure counts a full row for every computed distance instead)
             d_q, h_q = float(comp.sum(dtype=torch.int64).item()) / B, float(vis.sum(dtype=torch.int64).item()) / B
+            line["visited_members_per_query"] = round(h_q, 1)  # hops of the last step: divides the phases into per-hop cycles
             exact = d_q - ph["prefiltered"] + ph["survivors"]
             code = (a.dim + 15) // 16 * 16 + 16
             line["physical_bytes_per_query"] = round(exact * index.bytes_per_vector + ph["prefiltered"] * code + h_q * (4 + 4 * m0))

@@ -491,9 +491,21 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     uint32_t warps_sm = (uint32_t)std::min<size_t>(smem_sm / (fixed + min_heap + cta_tax), (size_t)search_max_warps_per_sm(d));
     if (forced_warps > 0) warps_sm = std::min<uint32_t>(warps_sm, (uint32_t)forced_warps);
     warps_sm = std::max(warps_sm, 1u);
-    uint32_t budget = (uint32_t)(smem_sm / warps_sm - cta_tax);
-    budget = std::min<uint32_t>(budget, (uint32_t)smem_cta_max);
-    uint32_t heap_bytes = std::min<uint32_t>((budget - fixed) & ~15u, 4096 * 8);
+    auto head_bytes = [&](uint32_t warps) { /* the shared memory left to the heap head at `warps` per SM */
+        uint32_t const budget = std::min<uint32_t>((uint32_t)(smem_sm / warps - cta_tax), (uint32_t)smem_cta_max);
+        return std::min<uint32_t>((budget - fixed) & ~15u, 4096 * 8);
+    };
+    /* Prefilter on: a hop is short, and a pop that leaves the warp-wide `pop_warp` (a head below the heap, which sends the
+     * pops to lane 0's serial walk and the HBM tail) is expensive. So plan for one warp per SM fewer when that lifts a head
+     * below PF_MIN_HEAP_HEAD entries. At 768-d (M=32, ef=128) a 7-warp budget leaves a 200-entry head, below the average
+     * per-query heap maximum of 353, and the 128-byte granularity of shared-memory allocation lets only 6 of those warps
+     * be resident anyway (792 blocks on 132 SMs); a 6-warp budget gives the same 6 warps an 896-entry head. 10M x 768 f32
+     * cosine on one H100 SXM at 400 W: 13.61 -> 12.77 ms per 4096-query launch (medians of three), heap_pop 0.63 M ->
+     * 0.31 M cycles per query (DESIGN §8). */
+    constexpr uint32_t PF_MIN_HEAP_HEAD = 512;
+    if (pl.prefilter && forced_warps <= 0 && tune.heap_head <= 0 && warps_sm > 2 && head_bytes(warps_sm) / 8 < PF_MIN_HEAP_HEAD)
+        warps_sm -= 1;
+    uint32_t heap_bytes = head_bytes(warps_sm);
     /* the heap_head knob: a smaller head sends more of the heap to its HBM tail; the root stays in shared memory */
     if (tune.heap_head > 0) heap_bytes = std::min<uint32_t>(heap_bytes, (uint32_t)std::max(tune.heap_head / 2, 1) * 16);
     pl.heap_smem_cap = heap_bytes / 8; /* even: heap_bytes is a multiple of 16 */

@@ -101,8 +101,8 @@ struct ip_f32_t {
     static constexpr bool NORMS = false;
     /* layer-0 prefilter through the int8 shadow (search_kernel.cu, measure_prefiltered; bound: prefilter_bound.h) */
     static constexpr bool PREFILTER = true;
-    static __device__ __forceinline__ double pf_lower(float dot, pf_record_t r, float a2, uint32_t n, float rho_a) {
-        return pf_ip_lower(dot, r.s, r.rho, a2, r.bnorm, n, rho_a);
+    static __device__ __forceinline__ double pf_lower(float dot, pf_record_t r, pf_query_bound_t const& q) {
+        return pf_ip_lower_q(dot, r.s, r.rho, r.bnorm, q);
     }
     template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
     template <class Q> static __device__ __forceinline__ float finalize_sw(float raw, Q, float) { return raw; }
@@ -130,8 +130,8 @@ struct cos_f32_t {
     static constexpr int LPV = 4;
     static constexpr bool NORMS = true;
     static constexpr bool PREFILTER = true; /* see ip_f32_t */
-    static __device__ __forceinline__ double pf_lower(float dot, pf_record_t r, float a2, uint32_t n, float rho_a) {
-        return pf_cos_lower(dot, r.s, r.rho, a2, r.b2, n, rho_a);
+    static __device__ __forceinline__ double pf_lower(float dot, pf_record_t r, pf_query_bound_t const& q) {
+        return pf_cos_lower_q(dot, r.s, r.rho, r.b2, q);
     }
     struct acc_t { float ab[4]; };
     struct qconst_t { float a2; };

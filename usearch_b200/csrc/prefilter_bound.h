@@ -111,6 +111,43 @@ PF_HD double pf_ip_lower(float dot, float s, float rho, float a2, float bnorm, u
     return 1.0 - ((double)s * (double)dot + A * (double)rho + T + delta);
 }
 
+/* The same two bounds with what depends only on the query (A = sqrt(a2), gamma_n and its products, the rho_a test)
+ * computed once per query: every candidate then runs the f64 operations above that involve its own record, on the same
+ * operands in the same order, so d_lo is the same bits. */
+struct pf_query_bound_t {
+    double A;      /* sqrt(a2) */
+    double gA;     /* pf_gamma(n) * A, the first product of pf_delta0 */
+    double n148;   /* n 2^-148, the first product of pf_delta0's underflow term */
+    double one_g;  /* 1 + pf_gamma(n) */
+    bool split_ok; /* rho_a is finite and not negative */
+    float rho_a;
+};
+
+PF_HD pf_query_bound_t pf_query_bound(float a2, uint32_t n, float rho_a) {
+    double const A = sqrt((double)a2), g = pf_gamma(n);
+    return pf_query_bound_t{A, g * A, (double)n * 0x1p-148, 1.0 + g, rho_a >= 0.0f && rho_a < INFINITY, rho_a};
+}
+
+PF_HD double pf_delta0_q(pf_query_bound_t const& q, double B, double s, double rho) {
+    return q.gA * (2.0 * B + 2.0 * rho) + q.n148 * (1.0 + s);
+}
+
+PF_HD double pf_cos_lower_q(float dot, float s, float rho, float b2, pf_query_bound_t const& q) {
+    double const A = q.A, B = sqrt((double)b2);
+    if (!pf_usable(A, B, s, rho) || !q.split_ok) return -INFINITY;
+    double const delta = PF_MARGIN * (pf_delta0_q(q, B, s, rho) + 0x1p-22 * A * B);
+    double const T = pf_split_term(q.rho_a, rho, B * q.one_g);
+    return 1.0 - ((double)s * (double)dot + A * (double)rho + T + delta) / (A * B);
+}
+
+PF_HD double pf_ip_lower_q(float dot, float s, float rho, float bnorm, pf_query_bound_t const& q) {
+    double const A = q.A, B = (double)bnorm;
+    if (!pf_usable(A, B, s, rho) || !q.split_ok) return -INFINITY;
+    double const delta = PF_MARGIN * (pf_delta0_q(q, B, s, rho) + 0x1p-24 * (1.0 + 2.0 * A * B));
+    double const T = pf_split_term(q.rho_a, rho, B);
+    return 1.0 - ((double)s * (double)dot + A * (double)rho + T + delta);
+}
+
 /* what the tightness checks compare against: d_ref - d_lo stays below this */
 PF_HD double pf_cos_gap_limit(float s, float rho, float a2, float b2, uint32_t n, float rho_a = 0.0f) {
     double const A = sqrt((double)a2), B = sqrt((double)b2);

@@ -127,25 +127,30 @@ struct heap_t {
 
     /*
      *  The same pop by the whole warp, for heaps whose internal nodes all sit in shared memory
-     *  (size <= 2*32*8 = 512 and size <= smem_cap). shift_down follows, from the root, the child chosen by
+     *  (size <= 2*32*WORDS and size < smem_cap). shift_down follows, from the root, the child chosen by
      *  `less`: right iff (right exists && right.d < left.d), else left — a choice that does not depend on
      *  the element being sifted — and stops at the first level where the sifted element is not worse
      *  (last.d > child.d fails); see index.hpp:819-834: `best` starts as last.d, moves to le.d if
      *  last.d > le.d, then to re.d if best > re.d, which is exactly "last.d > min-child.d, ties to the left".
-     *    1. every lane evaluates the choice bit of 8 internal nodes: one 16-byte load each, 8 ballots;
+     *    1. every lane evaluates the choice bit of up to WORDS internal nodes, one per 32-node word the heap reaches:
+     *       one 16-byte load and one ballot each;
      *    2. all lanes walk the <= 9 levels on those bits in registers (no memory on the critical path);
      *    3. lane k fetches the path node of level k, a ballot finds the stop level, the path shifts up.
      *  Returns false (nothing done) when the heap is too large: the caller falls back to `pop`.
+     *  WORDS = 8 (heaps up to 512 entries) or 16 (up to 1024: one more level of choice words). The prefiltered cos / ip
+     *  f32 search takes 16, because its plan gives the heap a head of at least 512 entries; every other kernel keeps 8,
+     *  whose smaller walk measured faster where heaps stay small (C1, l2sq 100K x 128: 1.53 against 1.57 ms per launch).
      */
-    __device__ __forceinline__ bool pop_warp(uint32_t size, int lane) const {
+    template <int WORDS> __device__ __forceinline__ bool pop_warp(uint32_t size, int lane) const {
+        static_assert(WORDS == 8 || WORDS == 16, "choice words: 8 or 16");
         uint32_t const n = size - 1;
         if (n == 0) return true;
-        if (size > 512u || size >= smem_cap) return false;
+        if (size > 64u * WORDS || size >= smem_cap) return false;
         cand_t const last = lds(smem_addr + 8u * size);
         uint32_t const internal = n >> 1; /* nodes 1..internal have at least a left child */
-        uint32_t w[8];
+        uint32_t w[WORDS];
 #pragma unroll
-        for (int r = 0; r < 8; ++r) {
+        for (int r = 0; r < WORDS; ++r) {
             w[r] = 0u;
             if ((uint32_t)(r * 32) <= internal) {
                 uint32_t const p = (uint32_t)(r * 32 + lane);
@@ -170,7 +175,10 @@ struct heap_t {
                 else if (k == 5) word = w[1];
                 else if (k == 6) word = (p & 32u) ? w[3] : w[2];
                 else if (k == 7) word = (p & 64u) ? ((p & 32u) ? w[7] : w[6]) : ((p & 32u) ? w[5] : w[4]);
-                else word = 0u; /* level-8 nodes (256..511) have no children when size <= 512 */
+                else if constexpr (WORDS == 8) word = 0u; /* level-8 nodes (256..511) have no children when size <= 512 */
+                else /* level 8 (level-9 nodes, 512..1023, have no children when size <= 1024) */
+                    word = (p & 128u) ? ((p & 64u) ? ((p & 32u) ? w[15] : w[14]) : ((p & 32u) ? w[13] : w[12]))
+                                      : ((p & 64u) ? ((p & 32u) ? w[11] : w[10]) : ((p & 32u) ? w[9] : w[8]));
                 uint32_t const child = 2u * p + ((word >> (p & 31u)) & 1u);
                 if (lane == k + 1) { mine = child; parent = p; }
                 p = child;
@@ -239,6 +247,8 @@ struct warp_ctx_t {
     uint32_t phase;      /* one parity bit per slot, uniform across the warp */
     uint32_t t_wait;     /* introspection: cycles spent waiting for staged vectors */
     uint32_t t_code;     /* introspection: cycles spent waiting for the prefilter's int8 codes */
+    uint32_t t_dot;      /* introspection: the prefilter's IMMA dot products and their conversion to `dot` */
+    uint32_t t_bound;    /* introspection: the prefilter's bound, ballots and compaction */
 };
 
 /* ---- distances of a whole candidate list ---------------------------------------------------- */
@@ -518,8 +528,8 @@ __device__ __forceinline__ void imma_16832(int (&c)[4], uint32_t a0, uint32_t a1
 
 template <class M>
 __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix, search_args_t const& a, warp_ctx_t& w,
-                                                     typename M::qconst_t qc, float a2, pf_query_split_t const& sp,
-                                                     float radius, uint32_t ncand, int lane) {
+                                                     typename M::qconst_t qc, pf_query_bound_t const& qb,
+                                                     pf_query_split_t const& sp, float radius, uint32_t ncand, int lane) {
     constexpr uint32_t MAX_TILES = 4; /* code_pass <= 64 */
     uint8_t* const smem = reinterpret_cast<uint8_t*>(w.q4); /* the query opens the warp's shared memory */
     float* const surv_b2 = reinterpret_cast<float*>(smem + a.off_surv_b2); /* cos: the survivors' stored squared norms */
@@ -555,32 +565,49 @@ __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix
         } else
             mbar_wait(bar, w.phase & 1u);
         w.phase ^= 1u;
+        long long const t_dot = a.phase_cycles ? clock64() : 0;
         /* k outer, tiles inner: one B load per k-step serves every tile. Rows of the last tile beyond `cnt` hold stale
          * bytes, and the k-bytes beyond `code_stride` of a row were never copied: the split is zero there, so they add 0
-         * to D1 and D2, and the rows' results are dropped. */
+         * to D1 and D2, and the rows' results are dropped.
+         * Even k-steps accumulate into acc[0], odd ones into acc[1], so that every tile has two independent chains of
+         * IMMAs; the s32 sums are exact, so D1 and D2 do not depend on the split. The fragments of step k + 1 are loaded
+         * before the IMMAs of step k issue. */
         uint32_t const ntiles = (cnt + 15) / 16;
-        int acc[MAX_TILES][4] = {};
-#pragma unroll 2
-        for (uint32_t k = 0; k < ksteps; ++k) {
-            uint32_t b0 = 0, b1 = 0;
-            if (lane < 8) asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(b0), "=r"(b1) : "r"(b_addr + 32u * k));
+        int acc[2][MAX_TILES][4] = {};
+        uint32_t fa[2][MAX_TILES][4], fb[2][2];
+        auto load = [&](uint32_t k, uint32_t(&A)[MAX_TILES][4], uint32_t(&B)[2]) {
+            B[0] = B[1] = 0u;
+            if (lane < 8) asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(B[0]), "=r"(B[1]) : "r"(b_addr + 32u * k));
 #pragma unroll
-            for (uint32_t t = 0; t < MAX_TILES; ++t) {
-                if (t < ntiles) { /* uniform */
-                    uint32_t a0, a1, a2r, a3;
-                    ldmatrix_x4(a_addr + t * 16u * scs + 32u * k, a0, a1, a2r, a3);
-                    imma_16832(acc[t], a0, a1, a2r, a3, b0, b1);
-                }
-            }
+            for (uint32_t t = 0; t < MAX_TILES; ++t)
+                if (t < ntiles) ldmatrix_x4(a_addr + t * 16u * scs + 32u * k, A[t][0], A[t][1], A[t][2], A[t][3]); /* uniform */
+        };
+        auto mma = [&](int (&C)[MAX_TILES][4], uint32_t const(&A)[MAX_TILES][4], uint32_t const(&B)[2]) {
+#pragma unroll
+            for (uint32_t t = 0; t < MAX_TILES; ++t)
+                if (t < ntiles) imma_16832(C[t], A[t][0], A[t][1], A[t][2], A[t][3], B[0], B[1]);
+        };
+        load(0, fa[0], fb[0]);
+        uint32_t k = 0;
+        for (; k + 2 <= ksteps; k += 2) { /* fa[0] holds step k */
+            load(k + 1, fa[1], fb[1]);
+            mma(acc[0], fa[0], fb[0]);
+            if (k + 2 < ksteps) load(k + 2, fa[0], fb[0]);
+            mma(acc[1], fa[1], fb[1]);
         }
+        if (k < ksteps) mma(acc[0], fa[0], fb[0]); /* an odd last step */
         /* C: lane 4 g holds columns 0 and 1 (D1, D2) of rows g and g + 8 */
 #pragma unroll
         for (uint32_t t = 0; t < MAX_TILES; ++t) {
             uint32_t const i = 16u * t + g;
-            if (sub == 0 && i < cnt) w.cand_d[base + i] = __double2float_rn(sa1 * (double)acc[t][0] + sa2 * (double)acc[t][1]);
-            if (sub == 0 && i + 8 < cnt) w.cand_d[base + i + 8] = __double2float_rn(sa1 * (double)acc[t][2] + sa2 * (double)acc[t][3]);
+            int const d1 = acc[0][t][0] + acc[1][t][0], d2 = acc[0][t][1] + acc[1][t][1];
+            int const d1h = acc[0][t][2] + acc[1][t][2], d2h = acc[0][t][3] + acc[1][t][3];
+            if (sub == 0 && i < cnt) w.cand_d[base + i] = __double2float_rn(sa1 * (double)d1 + sa2 * (double)d2);
+            if (sub == 0 && i + 8 < cnt) w.cand_d[base + i + 8] = __double2float_rn(sa1 * (double)d1h + sa2 * (double)d2h);
         }
         __syncwarp(); /* dots visible, and every lane is done with the stage area before it is refilled */
+        long long const t_bound = a.phase_cycles ? clock64() : 0;
+        if (a.phase_cycles) w.t_dot += (uint32_t)(t_bound - t_dot);
         uint32_t const lt = (1u << lane) - 1u;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -588,7 +615,7 @@ __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix
             if (32u * (uint32_t)h >= cnt) break; /* uniform */
             pf_record_t const r = h ? r1 : r0;
             bool keep = false;
-            if (i < cnt) keep = !(M::pf_lower(w.cand_d[c], r, a2, ix.dims, sp.rho_a) >= (double)radius);
+            if (i < cnt) keep = !(M::pf_lower(w.cand_d[c], r, qb) >= (double)radius);
             uint32_t const bal = __ballot_sync(0xffffffffu, keep);
             if (keep) { /* in place: ns + rank <= c, and the slots of this pass are in registers */
                 w.cand_s[ns + __popc(bal & lt)] = h ? s1 : s0;
@@ -597,6 +624,7 @@ __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix
             ns += __popc(bal);
         }
         __syncwarp();
+        if (a.phase_cycles) w.t_bound += (uint32_t)(clock64() - t_bound);
     }
     if (ns) {
         measure_staged<M>(ix, a, w, qc, ns, lane, w.cand_s, w.cand_d);
@@ -643,6 +671,8 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
     long long tp = prof ? clock64() : 0;
     w.t_wait = 0;
     w.t_code = 0;
+    w.t_dot = 0;
+    w.t_bound = 0;
 #define PHASE(acc)                                  \
     if (prof) {                                     \
         long long now_ = clock64();                 \
@@ -687,13 +717,14 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         __threadfence_block();
         __syncwarp();
         typename M::qconst_t qc = M::prepare(w.q4, ix.chunks16, lane);
-        float pf_a2 = 0.f; /* the query's squared norm, as the reference accumulates it */
         pf_query_split_t pf_sp{0.f, 0.f, INFINITY}; /* the query's int8 split, the B operand of the prefilter */
+        pf_query_bound_t pf_qb{};                   /* what the bound needs of the query alone */
         if constexpr (PF) {
-            pf_a2 = cos_f32_t::self_dot(w.q4, ix.chunks16, lane);
             if (a.prefilter) {
+                float const a2 = cos_f32_t::self_dot(w.q4, ix.chunks16, lane); /* as the reference accumulates it */
                 uint8_t* const q1 = reinterpret_cast<uint8_t*>(w.q4) + a.off_qsplit;
                 pf_sp = split_query(reinterpret_cast<float const*>(w.q4), ix.dims, q1, q1 + a.qsplit_len, a.qsplit_len, lane);
+                pf_qb = pf_query_bound(a2, ix.dims, pf_sp.rho_a);
             }
         }
         uint32_t const vmask = a.visited_cap - 1;
@@ -818,7 +849,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
                     if (s3 != EMPTY_SLOT) o3 = atomicOr(&visited[s3 >> 5], 1u << (s3 & 31));
                 }
             }
-            if (!heap.pop_warp(heap_size, lane)) {
+            if (!heap.template pop_warp<PF ? 16 : 8>(heap_size, lane)) {
                 if (lane == 0) heap.pop(heap_size);
             }
             heap_size -= 1;
@@ -910,7 +941,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
             uint32_t nacc = ncand; /* the candidates the accept replay visits */
             if constexpr (PF) {
                 if (a.prefilter && top_size == ef) { /* `top` full: every candidate must beat the radius */
-                    nacc = measure_prefiltered<M>(ix, a, w, qc, pf_a2, pf_sp, radius, ncand, lane);
+                    nacc = measure_prefiltered<M>(ix, a, w, qc, pf_qb, pf_sp, radius, ncand, lane);
                     n_pref += ncand;
                     n_surv += nacc;
                     measured = true;
@@ -1039,6 +1070,8 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         atomicAdd(a.phase_cycles + 11, (unsigned long long)n_pref);
         atomicAdd(a.phase_cycles + 12, (unsigned long long)n_surv);
         atomicAdd(a.phase_cycles + 13, (unsigned long long)w.t_code);
+        atomicAdd(a.phase_cycles + 14, (unsigned long long)w.t_dot);
+        atomicAdd(a.phase_cycles + 15, (unsigned long long)w.t_bound);
     }
 #undef PHASE
 }

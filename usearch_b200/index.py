@@ -534,7 +534,11 @@ class Index:
         q = max(int(out[7]), 1)
         return {"queries": int(out[7]), **{n: float(out[i]) / q for i, n in enumerate(names)},
                 "pushes": float(out[8]) / q, "avg_max_heap": float(out[9]) / q, "max_heap": int(out[10]),
-                "prefiltered": float(out[11]) / q, "survivors": float(out[12]) / q, "code_wait": float(out[13]) / q}
+                "prefiltered": float(out[11]) / q, "survivors": float(out[12]) / q, "code_wait": float(out[13]) / q,
+                "prefilter_dot": float(out[14]) / q, "prefilter_bound": float(out[15]) / q,
+                # what distance_math holds besides the prefilter: the survivors' FFMA pass and `finalize`, and whole
+                # lists measured without it (hops before `top` is full)
+                "survivor_math": float(out[4] - out[14] - out[15]) / q}
 
     # ---- sharded search: this index is one shard of a group of processes (shards.cu) ------------------------
     def join_shards(self, rank: int, world: int, unique_id: bytes) -> None:
