@@ -140,7 +140,7 @@ size_t usearch_search_many(usearch_index_t index, void const* queries, size_t qu
 /* usearch.h:338, c/lib.cpp:378-386 -> index_gt::add (index.hpp:2780-2880). The member is linked into the graph on the GPU
  * by the batched builder (csrc/builder.cu) — a batch of one here; usearch_b200_add_many below is the throughput entry.
  * Capacity grows on demand (the reference's C layer reports "Reserve capacity ahead of insertions!" instead). Removed
- * entries keep their slot (tombstone, skipped by searches); slots are not recycled. */
+ * entries keep their slot (tombstone, skipped by searches) until an add reuses it: see usearch_b200_change_reuse_removed. */
 void usearch_add(usearch_index_t index, usearch_key_t key, void const* vector, usearch_scalar_kind_t vector_kind, usearch_error_t* error); /* usearch.h:338 */
 bool usearch_contains(usearch_index_t index, usearch_key_t key, usearch_error_t* error);   /* usearch.h:349 */
 size_t usearch_count(usearch_index_t index, usearch_key_t key, usearch_error_t* error);    /* usearch.h:358 */
@@ -166,6 +166,25 @@ void usearch_b200_add_many(usearch_index_t index, usearch_key_t const* keys, voi
 /* The same with `keys` and `vectors` in DEVICE memory on the index's GPU. */
 void usearch_b200_add_many_device(usearch_index_t index, usearch_key_t const* keys, void const* vectors, size_t count,
                                   size_t vectors_stride, usearch_scalar_kind_t vector_kind, usearch_error_t* error);
+
+/* NEW (additive). Removal of many keys (python/lib.cpp:1210-1227 `remove_many`): every entry under each key becomes a
+ * tombstone and its slot joins a FIFO of removed slots (usearch_remove is this call with one key). Returns the number of
+ * entries removed. With `compact`, every link that leads to a removed entry is then erased on the GPU, on every level
+ * (index_dense_gt::isolate, index_dense.hpp:1709-1720); `pruned_edges` (may be NULL) receives the number of links erased.
+ * Removed entries keep their own links. */
+size_t usearch_b200_remove_many(usearch_index_t index, usearch_key_t const* keys, size_t count, bool compact,
+                                size_t* pruned_edges, usearch_error_t* error);
+/* NEW (additive). usearch_count for `count` keys at once (host only): counts[i] = entries stored under keys[i]; returns
+ * their sum. */
+size_t usearch_b200_count_many(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t* counts,
+                               usearch_error_t* error);
+/* NEW (additive). Slot reuse, off by default. When on, every add gives its i-th new entry the oldest removed slot while any
+ * is left (index_dense_gt::add_, index_dense.hpp:2020-2049) and appends the rest: the entry keeps the slot's level and
+ * rows, its lists are rebuilt by the INSERT search with its own slot kept out of its results (index_gt::update,
+ * index.hpp:2911-2999). Links that other entries still hold to the slot stay, as in the reference. When off, every add
+ * appends and removed slots are never reused. */
+void usearch_b200_change_reuse_removed(usearch_index_t index, bool reuse, usearch_error_t* error);
+bool usearch_b200_reuse_removed(usearch_index_t index);
 
 /* ---- additive: sharded search, one process per GPU (SURVEY.md §8e) ------------------------------------------------ */
 

@@ -280,11 +280,30 @@ __global__ void __launch_bounds__(LINK_THREADS, 3) link_reverse_kernel(__grid_co
         uint32_t const listed = count_shared;
         /* arrivals: the run of equal keys that starts at p0 (cut to what one refine can hold) */
         uint32_t const room = LINK_CAND_MAX - min(listed, LINK_CAND_MAX);
-        uint32_t arrivals = 0;
-        while (arrivals < room && p0 + arrivals < a.npairs && a.sorted_keys[p0 + arrivals] == key) ++arrivals; /* uniform */
+        uint32_t run = 0;
+        while (run < room && p0 + run < a.npairs && a.sorted_keys[p0 + run] == key) ++run; /* uniform */
+        /* An arrival that the list already holds is not appended again: a reused slot can still be listed from its
+         * previous life (the reference appends a second copy; the search kernel's visited test needs lists without
+         * repeats). `arrival` keeps the positions in the run of the others, in run order. */
+        uint32_t* const arrival = reinterpret_cast<uint32_t*>(smem + a.off_kept);
+        for (uint32_t i = threadIdx.x; i < run; i += blockDim.x) {
+            uint32_t const s = a.task_slot[a.sorted_idx[p0 + i] / ix.m];
+            bool listed_already = false;
+            for (uint32_t j = 0; j < listed && !listed_already; ++j) listed_already = row[j] == s;
+            arrival[i] = listed_already ? EMPTY_SLOT : p0 + i;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t fresh = 0;
+            for (uint32_t i = 0; i < run; ++i)
+                if (arrival[i] != EMPTY_SLOT) arrival[fresh++] = arrival[i];
+            count_shared = fresh;
+        }
+        __syncthreads();
+        uint32_t const arrivals = count_shared;
         if (listed + arrivals <= capacity) { /* close_header.push_back(new_slot), index.hpp:3871-3874 */
             for (uint32_t i = threadIdx.x; i < arrivals; i += blockDim.x) {
-                uint32_t const idx = a.sorted_idx[p0 + i];
+                uint32_t const idx = a.sorted_idx[arrival[i]];
                 row[listed + i] = a.task_slot[idx / ix.m];
             }
             continue;
@@ -295,13 +314,14 @@ __global__ void __launch_bounds__(LINK_THREADS, 3) link_reverse_kernel(__grid_co
             float d = __int_as_float(0x7f800000);
             if (i < listed) s = row[i];
             else if (i < listed + arrivals) {
-                uint32_t const idx = a.sorted_idx[p0 + (i - listed)];
+                uint32_t const idx = a.sorted_idx[arrival[i - listed]];
                 s = a.task_slot[idx / ix.m];
                 d = a.pair_dists[idx];
             }
             cs[i] = s;
             cd[i] = d;
         }
+        __syncthreads(); /* `arrival` shares its memory with the kept list of refine_block */
         fetch_vector(ix, centre, smem_u32(smem));
         cp_async_wait_all();
         __syncthreads();
@@ -482,6 +502,62 @@ __global__ void cast_rows_to_i8_kernel(uint8_t const* src, size_t src_stride, ui
     }
 }
 
+/* ---- removal and reuse: per-slot edits of `keys` / `deleted_bits`, rows scattered into reused slots ------------------ */
+
+/* new_keys == NULL: index_dense_gt::remove (index_dense.hpp:1479-1513), the slot takes the free key and its deleted bit;
+ * else the slot is reused under new_keys[i] and leaves the removed set */
+__global__ void edit_slots_kernel(uint32_t const* slots, uint32_t n, uint64_t const* new_keys, uint64_t free_key, uint64_t* keys,
+                                  uint32_t* deleted_bits) {
+    uint32_t const i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t const s = slots[i];
+    if (new_keys) {
+        keys[s] = new_keys[i];
+        atomicAnd(deleted_bits + (s >> 5), ~(1u << (s & 31)));
+    } else {
+        keys[s] = free_key;
+        atomicOr(deleted_bits + (s >> 5), 1u << (s & 31));
+    }
+}
+
+/* row i of `src` (already zero-padded to vec_stride) -> the row of slot slots[i] */
+__global__ void scatter_rows_kernel(uint4 const* src, uint32_t const* slots, uint32_t n, uint32_t chunks16, uint4* vectors) {
+    for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
+        uint4* dst = vectors + (size_t)slots[i] * chunks16;
+        for (uint32_t j = threadIdx.x; j < chunks16; j += blockDim.x) dst[j] = src[(size_t)i * chunks16 + j];
+    }
+}
+
+/* index_gt::isolate (index.hpp:3695-3728): one warp per list — the layer-0 rows of slots [0, n), then the upper rows in
+ * use — drops every link to a removed slot, keeps the survivors in stored order and fills the tail with EMPTY_SLOT. The
+ * dropped links are the reference's `pruned_edges`. Removed members keep their own links (the reference's comment at
+ * index.hpp:3684-3690). */
+__global__ void isolate_kernel(device_index_t const ix, uint32_t upper_rows, unsigned long long* pruned) {
+    uint32_t const lane = threadIdx.x & 31, lt = (1u << lane) - 1;
+    size_t const warps = (size_t)gridDim.x * (blockDim.x >> 5);
+    size_t const rows = (size_t)ix.n + upper_rows;
+    uint32_t dropped = 0;
+    for (size_t r = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < rows; r += warps) {
+        bool const base = r < ix.n;
+        uint32_t const width = base ? ix.m0 : ix.m;
+        uint32_t* const row = const_cast<uint32_t*>(base ? ix.nbr0 + r * ix.m0_stride : ix.upper + (r - ix.n) * ix.m_stride);
+        uint32_t kept = 0;
+        for (uint32_t b = 0; b < width; b += 32) {
+            uint32_t const s = b + lane < width ? row[b + lane] : EMPTY_SLOT;
+            bool const gone = s != EMPTY_SLOT && ((ix.deleted_bits[s >> 5] >> (s & 31)) & 1u);
+            bool const keep = s != EMPTY_SLOT && !gone;
+            uint32_t const bal = __ballot_sync(0xffffffffu, keep);
+            dropped += __popc(__ballot_sync(0xffffffffu, gone));
+            __syncwarp(); /* every lane has read its entry before the survivors move down */
+            if (keep) row[kept + __popc(bal & lt)] = s;
+            kept += __popc(bal);
+        }
+        __syncwarp();
+        for (uint32_t i = kept + lane; i < width; i += 32) row[i] = EMPTY_SLOT;
+    }
+    if (lane == 0 && dropped) atomicAdd(pruned, (unsigned long long)dropped);
+}
+
 uint64_t mix64(uint64_t x) { /* splitmix64 finaliser */
     x += 0x9E3779B97F4A7C15ull;
     x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -621,20 +697,78 @@ int16_t frozen_index_t::draw_level(size_t slot) const {
     return (int16_t)std::min<double>(r, 30.0);
 }
 
-/* Copy `count` vectors (host or device memory, any supported scalar kind) into the slab behind the current members, assign
- * keys and levels, and link them into the graph batch by batch. */
+/* `rows` caller vectors (host or device memory, any supported scalar kind) -> device rows of the index's scalar kind at
+ * `dst`, zero-padded to vec_stride; cast on the device when the kinds differ */
+char const* frozen_index_t::write_rows(void const* vectors, size_t rows, size_t stride, uint32_t kind, bool on_device, uint8_t* dst) {
+    if (!rows) return nullptr;
+    size_t const src_bytes = (dimensions * bits_per_scalar(kind) + 7) / 8;
+    if (kind == scalar) {
+        if (d.vec_stride != d.bytes_per_vector) CU(cudaMemsetAsync(dst, 0, rows * d.vec_stride, stream));
+        CU(cudaMemcpy2DAsync(dst, d.vec_stride, vectors, stride, d.bytes_per_vector, rows,
+                             on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
+        return nullptr;
+    }
+    size_t const chunk_rows = std::max<size_t>(1, (256u << 20) / std::max<size_t>(src_bytes, 1));
+    for (size_t lo = 0; lo < rows; lo += chunk_rows) {
+        size_t const n = std::min(chunk_rows, rows - lo);
+        uint8_t const* src = static_cast<uint8_t const*>(vectors) + lo * stride;
+        size_t src_stride = stride;
+        if (!on_device) {
+            if (char const* e = cast_stage.reserve(n * src_bytes)) return e;
+            CU(cudaMemcpy2DAsync(cast_stage.ptr, src_bytes, src, stride, src_bytes, n, cudaMemcpyHostToDevice, stream));
+            src = cast_stage.ptr;
+            src_stride = src_bytes;
+        }
+        if (char const* e = cast_rows_device(src, src_stride, kind, dst + lo * d.vec_stride, d.vec_stride, scalar, dimensions, n, stream))
+            return e;
+        CU(cudaStreamSynchronize(stream)); /* the staging buffer is reused by the next chunk */
+    }
+    return nullptr;
+}
+
+/* keys == NULL: mark `slots` removed; else give slot slots[i] the key keys[i] (host memory) and clear its deleted bit */
+char const* frozen_index_t::set_slot_keys(uint32_t const* slots, size_t count, uint64_t const* keys) {
+    if (!count) return nullptr;
+    if (!d.deleted_bits) {
+        uint32_t* bits = nullptr;
+        size_t const words = (capacity + 31) / 32;
+        CU(cudaMalloc(&bits, words * 4));
+        CU(cudaMemsetAsync(bits, 0, words * 4, stream));
+        dev_allocs[5] = bits;
+        d.deleted_bits = bits;
+        hbm_bytes += words * 4;
+    }
+    if (char const* e = edit_slots.reserve(count)) return e;
+    CU(cudaMemcpyAsync(edit_slots.ptr, slots, count * 4, cudaMemcpyHostToDevice, stream));
+    if (keys) {
+        if (char const* e = edit_keys.reserve(count)) return e;
+        CU(cudaMemcpyAsync(edit_keys.ptr, keys, count * 8, cudaMemcpyHostToDevice, stream));
+    }
+    edit_slots_kernel<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(edit_slots.ptr, (uint32_t)count, keys ? edit_keys.ptr : nullptr,
+                                                                           free_key, const_cast<uint64_t*>(d.keys),
+                                                                           const_cast<uint32_t*>(d.deleted_bits));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(stream)); /* `slots` / `keys` are the caller's pageable memory */
+    return nullptr;
+}
+
+/* Store `count` vectors (host or device memory, any supported scalar kind), assign keys and levels, and link them into the
+ * graph batch by batch. With `reuse_removed`, the first of them take the oldest removed slots (index_dense_gt::add_,
+ * index_dense.hpp:2020-2049, then index_gt::update, index.hpp:2911-2999) and only the rest are appended. */
 char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vectors, size_t count, size_t stride, uint32_t kind,
                                      bool on_device) {
     if (!count) return nullptr;
     if (char const* e = ensure_context()) return e;
     if (!configured()) return "Index is not initialized: call usearch_init with options or load a file first";
     if (!bits_per_scalar(kind)) return "Unknown scalar kind!";
+    size_t const reused = reuse_removed ? std::min(count, free_slots.size()) : 0;
+    size_t const appended = count - reused;
     size_t const first = size;
-    if (first + count >= 0xFFFFFFFFull) return "Too many entries for 32-bit slots";
-    if (first + count > capacity) {
+    if (first + appended >= 0xFFFFFFFFull) return "Too many entries for 32-bit slots";
+    if (first + appended > capacity) {
         /* c/lib.cpp leaves growth to the caller ("Reserve capacity ahead of insertions!", index.hpp:2816); the Python binding
          * grows by powers of two (python/lib.cpp:203-208) — here the library does the same on its own */
-        size_t want = std::max<size_t>(first + count, capacity * 2);
+        size_t want = std::max<size_t>(first + appended, capacity * 2);
         if (char const* e = reserve_slots(want)) return e;
     }
     std::vector<uint64_t> keys_copy;
@@ -657,54 +791,61 @@ char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vecto
     }
     size_t const src_bytes = (dimensions * bits_per_scalar(kind) + 7) / 8;
     if (stride == 0) stride = src_bytes;
+    uint8_t const* const appended_vectors = static_cast<uint8_t const*>(vectors) + reused * stride;
 
-    /* vectors -> slab rows [first, first + count), cast on the device when the caller's scalar kind differs */
+    /* reused slots: the new rows are staged, scattered into their slots, and their norms / int8 shadow recomputed */
+    std::vector<uint32_t> reuse_slots(free_slots.begin(), free_slots.begin() + (ptrdiff_t)reused);
+    if (reused) {
+        if (char const* e = reuse_stage.reserve(reused * d.vec_stride)) return e;
+        if (char const* e = write_rows(vectors, reused, stride, kind, on_device, reuse_stage.ptr)) return e;
+        if (char const* e = edit_slots.reserve(reused)) return e;
+        CU(cudaMemcpyAsync(edit_slots.ptr, reuse_slots.data(), reused * 4, cudaMemcpyHostToDevice, stream));
+        scatter_rows_kernel<<<(unsigned)std::min<size_t>(reused, 65535), 128, 0, stream>>>(
+            reinterpret_cast<uint4 const*>(reuse_stage.ptr), edit_slots.ptr, (uint32_t)reused, d.chunks16,
+            reinterpret_cast<uint4*>(const_cast<uint8_t*>(d.vectors)));
+        CU(cudaGetLastError());
+        device_index_t part = d;
+        part.n = (uint32_t)reused;
+        if (d.norms) CU(search_compute_norms(part, const_cast<float*>(d.norms), stream, edit_slots.ptr));
+        if (d.codes) /* after the norms: the records copy them */
+            CU(search_compute_shadow(part, d.norms, const_cast<int8_t*>(d.codes), const_cast<pf_record_t*>(d.shadow), stream,
+                                     edit_slots.ptr));
+        CU(cudaStreamSynchronize(stream));
+        free_slots.erase(free_slots.begin(), free_slots.begin() + (ptrdiff_t)reused);
+    }
+
+    /* appended: vectors -> slab rows [first, first + appended) */
     uint8_t* slab = const_cast<uint8_t*>(d.vectors) + first * d.vec_stride;
-    size_t const chunk_rows = std::max<size_t>(1, (256u << 20) / std::max<size_t>(src_bytes, 1));
-    if (kind == scalar) {
-        if (d.vec_stride != d.bytes_per_vector) CU(cudaMemsetAsync(slab, 0, count * d.vec_stride, stream));
-        CU(cudaMemcpy2DAsync(slab, d.vec_stride, vectors, stride, d.bytes_per_vector, count,
-                             on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
-    } else {
-        for (size_t lo = 0; lo < count; lo += chunk_rows) {
-            size_t const rows = std::min(chunk_rows, count - lo);
-            uint8_t const* src = static_cast<uint8_t const*>(vectors) + lo * stride;
-            size_t src_stride = stride;
-            if (!on_device) {
-                if (char const* e = cast_stage.reserve(rows * src_bytes)) return e;
-                CU(cudaMemcpy2DAsync(cast_stage.ptr, src_bytes, src, stride, src_bytes, rows, cudaMemcpyHostToDevice, stream));
-                src = cast_stage.ptr;
-                src_stride = src_bytes;
-            }
-            if (char const* e = cast_rows_device(src, src_stride, kind, slab + lo * d.vec_stride, d.vec_stride, scalar, dimensions, rows, stream))
-                return e;
-            CU(cudaStreamSynchronize(stream)); /* the staging buffer is reused by the next chunk */
+    if (appended) {
+        if (char const* e = write_rows(appended_vectors, appended, stride, kind, on_device, slab)) {
+            free_slots.insert(free_slots.begin(), reuse_slots.begin(), reuse_slots.end());
+            return e;
         }
+        CU(cudaMemcpyAsync(const_cast<uint64_t*>(d.keys) + first, new_keys + reused, appended * 8,
+                           on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
+        if (d.norms) {
+            device_index_t part = d;
+            part.vectors = slab;
+            part.n = (uint32_t)appended;
+            CU(search_compute_norms(part, const_cast<float*>(d.norms) + first, stream));
+        }
+        if (d.codes) { /* after the norms: the records copy them */
+            device_index_t part = d;
+            part.vectors = slab;
+            part.n = (uint32_t)appended;
+            CU(search_compute_shadow(part, d.norms ? d.norms + first : nullptr, const_cast<int8_t*>(d.codes) + first * d.code_stride,
+                                     const_cast<pf_record_t*>(d.shadow) + first, stream));
+        }
+        CU(cudaStreamSynchronize(stream)); /* `vectors` / `new_keys` may be pageable host memory owned by the caller */
     }
-    CU(cudaMemcpyAsync(const_cast<uint64_t*>(d.keys) + first, new_keys, count * 8,
-                       on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
-    if (d.norms) {
-        device_index_t part = d;
-        part.vectors = slab;
-        part.n = (uint32_t)count;
-        CU(search_compute_norms(part, const_cast<float*>(d.norms) + first, stream));
-    }
-    if (d.codes) { /* after the norms: the records copy them */
-        device_index_t part = d;
-        part.vectors = slab;
-        part.n = (uint32_t)count;
-        CU(search_compute_shadow(part, d.norms ? d.norms + first : nullptr, const_cast<int8_t*>(d.codes) + first * d.code_stride,
-                                 const_cast<pf_record_t*>(d.shadow) + first, stream));
-    }
-    CU(cudaStreamSynchronize(stream)); /* `vectors` / `new_keys` may be pageable host memory owned by the caller */
 
-    /* host-side bookkeeping: keys, levels, rows in `upper` */
-    host_keys.reserve(first + count);
-    levels.reserve(first + count);
-    std::vector<uint32_t> bases(count);
+    /* host-side bookkeeping of the appended members: keys, levels, rows in `upper` */
+    host_keys.reserve(first + appended);
+    levels.reserve(first + appended);
+    std::vector<uint32_t> bases(appended);
     size_t rows = upper_rows;
-    host_keys.insert(host_keys.end(), hk, hk + count);
-    for (size_t i = 0; i < count; ++i) {
+    host_keys.insert(host_keys.end(), hk + reused, hk + count);
+    for (size_t i = 0; i < appended; ++i) {
         int16_t const level = draw_level(first + i);
         levels.push_back(level);
         bases[i] = level ? (uint32_t)rows : EMPTY_SLOT;
@@ -713,15 +854,51 @@ char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vecto
     if (rows >= 0xFFFFFFFFull) return "Too many upper-level rows";
     if (char const* e = reserve_upper_rows(rows)) return e;
     upper_rows = rows;
-    CU(cudaMemcpyAsync(const_cast<uint32_t*>(d.upper_base) + first, bases.data(), count * 4, cudaMemcpyHostToDevice, stream));
-    CU(cudaStreamSynchronize(stream));
+    if (appended) {
+        CU(cudaMemcpyAsync(const_cast<uint32_t*>(d.upper_base) + first, bases.data(), appended * 4, cudaMemcpyHostToDevice, stream));
+        CU(cudaStreamSynchronize(stream));
+    }
     if (key_map.built)
-        for (size_t i = 0; i < count; ++i) key_map.insert(host_keys[first + i], (uint32_t)(first + i));
-    size = first + count; /* stored; `d.n` counts the members that are linked into the graph */
+        for (size_t i = 0; i < appended; ++i) key_map.insert(host_keys[first + i], (uint32_t)(first + i));
+    size = first + appended; /* stored; `d.n` counts the members that are linked into the graph */
 
-    /* link them, batch by batch */
+    /* link them, batch by batch: the reused slots first, then the appended ones */
     static size_t const batch_max = [] { char const* v = std::getenv("USEARCH_B200_BUILD_BATCH"); return v && std::atol(v) > 0 ? (size_t)std::atol(v) : (size_t)32768; }();
     static size_t const ratio = [] { char const* v = std::getenv("USEARCH_B200_BUILD_RATIO"); return v && std::atol(v) > 0 ? (size_t)std::atol(v) : (size_t)32; }();
+    auto drop_unlinked = [&](size_t reused_linked) {
+        /* reused slots that were not linked go back to the front of the queue and stay removed; members that were
+         * stored but not linked are dropped again: the index stays what the graph says it is */
+        free_slots.insert(free_slots.begin(), reuse_slots.begin() + (ptrdiff_t)reused_linked, reuse_slots.end());
+        size_t rows_kept = 0;
+        for (size_t i = 0; i < (size_t)d.n; ++i) rows_kept += (size_t)levels[i];
+        size = d.n;
+        host_keys.resize(size);
+        levels.resize(size);
+        upper_rows = rows_kept;
+        key_map.clear();
+        cudaMemsetAsync(const_cast<uint32_t*>(d.nbr0) + size * d.m0_stride, 0xFF, (first + appended - size) * d.m0_stride * 4, stream);
+        if (upper_capacity > upper_rows)
+            cudaMemsetAsync(const_cast<uint32_t*>(d.upper) + upper_rows * d.m_stride, 0xFF, (upper_capacity - upper_rows) * d.m_stride * 4, stream);
+        cudaStreamSynchronize(stream);
+    };
+    for (size_t at = 0; at < reused;) {
+        /* a reused member keeps its level (<= the top level) and its rows: it never ends a batch */
+        size_t const batch = std::min<size_t>({reused - at, batch_max, std::max<size_t>((size_t)d.n / ratio, 1)});
+        char const* e = link_batch(reuse_slots.data() + at, batch);
+        if (!e) e = set_slot_keys(reuse_slots.data() + at, batch, hk + at);
+        if (e) {
+            drop_unlinked(at);
+            return e;
+        }
+        build_key_map();
+        for (size_t i = at; i < at + batch; ++i) {
+            host_keys[reuse_slots[i]] = hk[i];
+            key_map.insert(hk[i], reuse_slots[i]);
+        }
+        count_deleted -= batch;
+        at += batch;
+    }
+    std::vector<uint32_t> batch_slots;
     size_t at = first;
     while (at < size) {
         if (d.n == 0) { /* the first member: entry point, no links (index.hpp:2836-2841) */
@@ -735,19 +912,10 @@ char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vecto
         /* a member above the current top level ends its batch: the next batch descends from it */
         for (size_t i = 0; i < batch; ++i)
             if (levels[at + i] > d.max_level) { batch = i + 1; break; }
-        if (char const* e = link_batch(at, batch)) {
-            /* members that were stored but not linked are dropped again: the index stays what the graph says it is */
-            size_t rows_kept = 0;
-            for (size_t i = 0; i < (size_t)d.n; ++i) rows_kept += (size_t)levels[i];
-            size = d.n;
-            host_keys.resize(size);
-            levels.resize(size);
-            upper_rows = rows_kept;
-            key_map.clear();
-            cudaMemsetAsync(const_cast<uint32_t*>(d.nbr0) + size * d.m0_stride, 0xFF, (first + count - size) * d.m0_stride * 4, stream);
-            if (upper_capacity > upper_rows)
-                cudaMemsetAsync(const_cast<uint32_t*>(d.upper) + upper_rows * d.m_stride, 0xFF, (upper_capacity - upper_rows) * d.m_stride * 4, stream);
-            cudaStreamSynchronize(stream);
+        batch_slots.resize(batch);
+        for (size_t i = 0; i < batch; ++i) batch_slots[i] = (uint32_t)(at + i);
+        if (char const* e = link_batch(batch_slots.data(), batch)) {
+            drop_unlinked(reused);
             return e;
         }
         at += batch;
@@ -755,8 +923,9 @@ char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vecto
     return nullptr;
 }
 
-/* steps 1-4 of the header comment for the members in slots [first, first + count) */
-char const* frozen_index_t::link_batch(size_t first, size_t count) {
+/* steps 1-4 of the header comment for the members in `slots`: appended slots (>= d.n, in order), or reused slots whose
+ * rows are rewritten on every level they own */
+char const* frozen_index_t::link_batch(uint32_t const* slots, size_t count) {
     cudaStream_t const s = stream;
     uint32_t const top_level = (uint32_t)d.max_level;
     /* work items: level 0 of every member first (the long searches start first), then the upper levels */
@@ -764,13 +933,14 @@ char const* frozen_index_t::link_batch(size_t first, size_t count) {
     std::vector<uint8_t> t_level;
     t_slot.reserve(count + count / 8 + 8);
     t_level.reserve(count + count / 8 + 8);
-    for (size_t i = 0; i < count; ++i) { t_slot.push_back((uint32_t)(first + i)); t_level.push_back(0); }
+    for (size_t i = 0; i < count; ++i) { t_slot.push_back(slots[i]); t_level.push_back(0); }
     int16_t new_top = d.max_level;
-    uint32_t new_entry = d.entry_slot;
+    uint32_t new_entry = d.entry_slot, new_n = d.n;
     for (size_t i = 0; i < count; ++i) {
-        int16_t const level = levels[first + i];
-        for (uint32_t l = 1; l <= std::min<uint32_t>((uint32_t)level, top_level); ++l) { t_slot.push_back((uint32_t)(first + i)); t_level.push_back((uint8_t)l); }
-        if (level > new_top) { new_top = level; new_entry = (uint32_t)(first + i); }
+        int16_t const level = levels[slots[i]];
+        for (uint32_t l = 1; l <= std::min<uint32_t>((uint32_t)level, top_level); ++l) { t_slot.push_back(slots[i]); t_level.push_back((uint8_t)l); }
+        if (level > new_top) { new_top = level; new_entry = slots[i]; }
+        new_n = std::max(new_n, slots[i] + 1);
     }
     size_t const ntasks = t_slot.size();
     uint32_t const ef = (uint32_t)std::max<size_t>(expansion_add ? expansion_add : 128, 1);
@@ -876,9 +1046,58 @@ char const* frozen_index_t::link_batch(size_t first, size_t count) {
     kernel_launches += 3;
     CU(cudaStreamSynchronize(s));
 
-    d.n = (uint32_t)(first + count);
+    d.n = new_n;
     d.max_level = new_top;
     d.entry_slot = new_entry;
+    return nullptr;
+}
+
+/* ---------------------------------------------------------------------------------------------------------------------- */
+/*  remove                                                                                                                  */
+/* ---------------------------------------------------------------------------------------------------------------------- */
+
+/* index_dense_gt::remove over many keys (index_dense.hpp:1515-1557): each entry keeps its node and its links, its key becomes
+ * the free key (so searches skip it: `deleted_bits`), the key leaves the lookup table, and the slot joins `free_slots`.
+ * With `compact`, links that lead to removed entries are then pruned (python/lib.cpp:1210-1227 -> isolate). */
+char const* frozen_index_t::remove_many(uint64_t const* keys, size_t count, bool compact, size_t* removed, size_t* pruned) {
+    *removed = 0;
+    if (pruned) *pruned = 0;
+    if (!loaded || !size) return nullptr;
+    if (char const* e = ensure_context()) return e;
+    build_key_map();
+    std::vector<uint32_t> slots;
+    for (size_t i = 0; i < count; ++i) {
+        size_t const before = slots.size();
+        key_map.for_each(keys[i], [&](uint32_t slot, size_t cell) { slots.push_back(slot); key_map.erase_cell(cell); return true; });
+        std::sort(slots.begin() + (ptrdiff_t)before, slots.end()); /* the entries of one key of a multi index: insertion order */
+    }
+    if (char const* e = set_slot_keys(slots.data(), slots.size(), nullptr)) {
+        key_map.clear(); /* rebuilt from host_keys, which still hold the keys */
+        return e;
+    }
+    for (uint32_t slot : slots) {
+        host_keys[slot] = free_key;
+        free_slots.push_back(slot);
+    }
+    count_deleted += slots.size();
+    *removed = slots.size();
+    if (!compact) return nullptr;
+    return isolate(pruned);
+}
+
+char const* frozen_index_t::isolate(size_t* pruned) {
+    if (pruned) *pruned = 0;
+    if (!d.deleted_bits || !d.n) return nullptr; /* nothing was ever removed */
+    if (char const* e = pruned_counter.reserve(1)) return e;
+    CU(cudaMemsetAsync(pruned_counter.ptr, 0, 8, stream));
+    size_t const rows = (size_t)d.n + upper_rows;
+    unsigned const blocks = (unsigned)std::min<size_t>((rows + 7) / 8, (size_t)sm_count * 8);
+    isolate_kernel<<<blocks, 256, 0, stream>>>(d, (uint32_t)upper_rows, pruned_counter.ptr);
+    CU(cudaGetLastError());
+    unsigned long long total = 0;
+    CU(cudaMemcpyAsync(&total, pruned_counter.ptr, 8, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    if (pruned) *pruned = (size_t)total;
     return nullptr;
 }
 

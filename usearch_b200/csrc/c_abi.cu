@@ -434,12 +434,38 @@ size_t usearch_get(usearch_index_t index, usearch_key_t key, size_t count, void*
 }
 
 size_t usearch_remove(usearch_index_t index, usearch_key_t key, usearch_error_t* error) { /* c/lib.cpp:439-446 */
+    return usearch_b200_remove_many(index, &key, 1, false, nullptr, error);
+}
+
+size_t usearch_b200_remove_many(usearch_index_t index, usearch_key_t const* keys, size_t count, bool compact,
+                                size_t* pruned_edges, usearch_error_t* error) {
     frozen_index_t* ix = as_index(index);
     std::lock_guard<std::mutex> lock(ix->mutex);
     size_t removed = 0;
-    set_error(error, guarded([&] { return ix->remove_key(key, &removed); }));
+    set_error(error, guarded([&] { return ix->remove_many(keys, count, compact, &removed, pruned_edges); }));
     return removed;
 }
+
+size_t usearch_b200_count_many(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t* counts, usearch_error_t*) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    ix->build_key_map();
+    size_t total = 0;
+    for (size_t i = 0; i < count; ++i) {
+        size_t const c = ix->key_map.count(keys[i]);
+        if (counts) counts[i] = c;
+        total += c;
+    }
+    return total;
+}
+
+void usearch_b200_change_reuse_removed(usearch_index_t index, bool reuse, usearch_error_t*) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    ix->reuse_removed = reuse;
+}
+
+bool usearch_b200_reuse_removed(usearch_index_t index) { return as_index(index)->reuse_removed; }
 
 size_t usearch_rename(usearch_index_t index, usearch_key_t from, usearch_key_t to, usearch_error_t* error) { /* c/lib.cpp:448-455 */
     frozen_index_t* ix = as_index(index);

@@ -91,6 +91,7 @@ void frozen_index_t::release_device() {
     loaded = false;
     size = 0;
     count_deleted = 0;
+    free_slots.clear();
     capacity = 0;
     upper_capacity = 0;
     upper_rows = 0;
@@ -346,6 +347,9 @@ char const* frozen_index_t::load_blob(uint8_t const* blob, size_t length) {
     }
     drop_host_state.armed = false;
     commit(ix, upper_rows);
+    /* reindex_keys_ (index_dense.hpp:2160-2188): removed slots queue up for reuse in ascending order */
+    for (uint64_t i = 0; i < n; ++i)
+        if (host_keys[i] == free_key) free_slots.push_back((uint32_t)i);
     return nullptr;
 }
 
@@ -1083,38 +1087,6 @@ char const* pair_distance_host(void const* a, void const* b, uint32_t scalar, si
 /* ---------------------------------------------------------------------------------------------- */
 /*  lookups and edits by key                                                                      */
 /* ---------------------------------------------------------------------------------------------- */
-
-/* index_dense_gt::remove (index_dense.hpp:1480-1513): the entry keeps its node and its links, its key becomes the free key
- * (so searches skip it: `deleted_bits`), and the key leaves the lookup table. Slots are not recycled. */
-char const* frozen_index_t::remove_key(uint64_t key, size_t* removed) {
-    *removed = 0;
-    if (!loaded || !size) return nullptr;
-    if (char const* e = ensure_context()) return e;
-    build_key_map();
-    std::vector<uint32_t> slots;
-    key_map.for_each(key, [&](uint32_t slot, size_t cell) { slots.push_back(slot); key_map.erase_cell(cell); return true; });
-    if (slots.empty()) return nullptr;
-    if (!d.deleted_bits) {
-        uint32_t* bits = nullptr;
-        size_t const words = (capacity + 31) / 32;
-        CU(cudaMalloc(&bits, words * 4));
-        CU(cudaMemset(bits, 0, words * 4));
-        dev_allocs[5] = bits;
-        d.deleted_bits = bits;
-        hbm_bytes += words * 4;
-    }
-    for (uint32_t slot : slots) {
-        host_keys[slot] = free_key;
-        CU(cudaMemcpy(const_cast<uint64_t*>(d.keys) + slot, &free_key, 8, cudaMemcpyHostToDevice));
-        uint32_t word = 0;
-        CU(cudaMemcpy(&word, d.deleted_bits + (slot >> 5), 4, cudaMemcpyDeviceToHost));
-        word |= 1u << (slot & 31);
-        CU(cudaMemcpy(const_cast<uint32_t*>(d.deleted_bits) + (slot >> 5), &word, 4, cudaMemcpyHostToDevice));
-    }
-    count_deleted += slots.size();
-    *removed = slots.size();
-    return nullptr;
-}
 
 /* index_dense_gt::rename (index_dense.hpp:1554-1580): every entry under `from` gets the key `to` */
 char const* frozen_index_t::rename_key(uint64_t from, uint64_t to, size_t* renamed) {

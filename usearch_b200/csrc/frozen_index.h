@@ -10,6 +10,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <condition_variable>
+#include <deque>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -31,11 +32,12 @@ uint32_t search_stage_pad(device_index_t const& ix);
 int search_max_warps_per_sm(device_index_t const& ix);
 bool search_single_stage_set(device_index_t const& ix);
 bool search_needs_norms(uint32_t metric, uint32_t scalar);
-cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStream_t stream);
+/* `slots` (optional, ix.n entries): recompute only those rows of the full arrays instead of rows 0 .. ix.n-1 */
+cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStream_t stream, uint32_t const* slots = nullptr);
 bool search_needs_shadow(device_index_t const& ix);
 uint32_t search_code_stride(device_index_t const& ix);
 cudaError_t search_compute_shadow(device_index_t const& ix, float const* norms, int8_t* codes, pf_record_t* records,
-                                  cudaStream_t stream);
+                                  cudaStream_t stream, uint32_t const* slots = nullptr);
 cudaError_t search_fill_empty(uint64_t* keys, float* dists, uint32_t* counts, uint32_t* computed, uint32_t* visited, size_t nq,
                               size_t k, cudaStream_t stream);
 cudaError_t search_build_allow_bits(device_index_t const& ix, uint64_t const* allowed_sorted, uint32_t m, uint32_t* bits,
@@ -136,6 +138,10 @@ struct frozen_index_t {
     std::vector<int16_t> levels;     /* kept on the host: re-serialisation and the builder's work lists */
     std::vector<uint64_t> host_keys; /* host copy of `keys` (slot -> key): lookups by key never touch the device */
     key_map_t key_map;
+    /* removed slots awaiting reuse, oldest first: the reference's `free_keys_` ring (index.hpp:1308-1330) pushes at the
+     * head and pops from the tail. `remove` appends in removal order; a load refills it in ascending slot order. */
+    std::deque<uint32_t> free_slots;
+    bool reuse_removed = false; /* add() fills `free_slots` before appending (off: every add appends, as before) */
     size_t capacity = 0;                      /* slots the HBM arrays have room for */
     size_t upper_capacity = 0, upper_rows = 0; /* rows of `upper`: allocated / in use */
     uint64_t level_seed = 0;
@@ -204,8 +210,16 @@ struct frozen_index_t {
     char const* reserve_upper_rows(size_t rows);
     int16_t draw_level(size_t slot) const;
     char const* add_many(uint64_t const* keys, void const* vectors, size_t count, size_t stride, uint32_t scalar_kind, bool on_device);
-    char const* link_batch(size_t first, size_t count);
-    char const* remove_key(uint64_t key, size_t* removed);
+    char const* link_batch(uint32_t const* slots, size_t count);
+    /* remove / reuse: the slots of one call and the keys they take, uploaded once; reused rows staged before the scatter */
+    device_buffer_t<uint32_t> edit_slots;
+    device_buffer_t<uint64_t> edit_keys;
+    device_buffer_t<uint8_t> reuse_stage;
+    device_buffer_t<unsigned long long> pruned_counter;
+    char const* write_rows(void const* vectors, size_t rows, size_t stride, uint32_t kind, bool on_device, uint8_t* dst);
+    char const* set_slot_keys(uint32_t const* slots, size_t count, uint64_t const* keys);
+    char const* remove_many(uint64_t const* keys, size_t count, bool compact, size_t* removed, size_t* pruned);
+    char const* isolate(size_t* pruned);
     char const* rename_key(uint64_t from, uint64_t to, size_t* renamed);
     char const* get_vectors(uint64_t key, size_t max_count, void* out, uint32_t out_scalar, size_t* found);
 

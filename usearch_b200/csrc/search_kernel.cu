@@ -808,7 +808,9 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         PHASE(pc0)
         {
             /* cluster(): the closest member at that level is the whole answer, predicate ignored (index.hpp:3122) */
-            bool allowed = cluster || insert || slot_allowed(ix, a, closest);
+            /* search_to_update_ (index.hpp:4086-4168): a reused slot is searched from and expanded, but never
+             * enters its own `top`. For an appended member no list reaches its slot, so the test never fires. */
+            bool allowed = cluster || (insert ? closest != qi : slot_allowed(ix, a, closest));
             if (allowed) {
                 if (topreg) {
                     if (lane == 0) { rtd[0] = radius; rts[0] = closest; }
@@ -968,7 +970,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
                         heap.push(heap_size, cand_t{d, s}, lane);
                         heap_size += 1;
                         if (prof) { n_push += 1; max_heap = max(max_heap, heap_size); }
-                        bool allowed = insert || slot_allowed(ix, a, s);
+                        bool allowed = insert ? s != qi : slot_allowed(ix, a, s);
                         if (allowed) {
                             if (topreg) {
                                 top_insert_reg(rtd, rts, top_size, ef, d, s, lane);
@@ -1163,29 +1165,30 @@ cudaError_t search_build_allow_bits(device_index_t const& ix, uint64_t const* al
 
 /* ---- freeze-time helper: squared norms in the metric's summation order -------------------------- */
 
-template <class M> __global__ void norms_kernel(device_index_t ix, float* norms) {
+template <class M> __global__ void norms_kernel(device_index_t ix, float* norms, uint32_t const* slots) {
     constexpr int LPV = M::LPV;
     uint32_t const lane = threadIdx.x & 31, group = (blockIdx.x * blockDim.x + threadIdx.x) / LPV;
-    uint32_t const slot = group < ix.n ? group : ix.n - 1; /* whole warps stay converged for the shuffles */
+    uint32_t const i = group < ix.n ? group : ix.n - 1; /* whole warps stay converged for the shuffles */
+    uint32_t const slot = slots ? slots[i] : i;
     uint4 const* v = reinterpret_cast<uint4 const*>(ix.vectors + (size_t)slot * ix.vec_stride);
     float b2 = M::self_dot(v, ix.chunks16, (int)lane);
-    if (group < ix.n && (lane % LPV) == 0) norms[group] = b2;
+    if (group < ix.n && (lane % LPV) == 0) norms[slot] = b2;
 }
 
 bool search_needs_norms(uint32_t metric, uint32_t scalar) {
     return metric == METRIC_COS && (scalar == SCALAR_F32 || scalar == SCALAR_F16 || scalar == SCALAR_BF16);
 }
 
-cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStream_t stream) {
+cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStream_t stream, uint32_t const* slots) {
     if (!ix.n) return cudaSuccess;
     uint32_t const threads = 256;
     if (ix.scalar == SCALAR_F32) {
         uint32_t const per_block = threads / 4;
-        norms_kernel<cos_f32_t><<<(ix.n + per_block - 1) / per_block, threads, 0, stream>>>(ix, norms);
+        norms_kernel<cos_f32_t><<<(ix.n + per_block - 1) / per_block, threads, 0, stream>>>(ix, norms, slots);
     } else if (ix.scalar == SCALAR_F16) {
-        norms_kernel<cos_half_t<f16_conv_t>><<<(ix.n + threads - 1) / threads, threads, 0, stream>>>(ix, norms);
+        norms_kernel<cos_half_t<f16_conv_t>><<<(ix.n + threads - 1) / threads, threads, 0, stream>>>(ix, norms, slots);
     } else if (ix.scalar == SCALAR_BF16) {
-        norms_kernel<cos_half_t<bf16_conv_t>><<<(ix.n + threads - 1) / threads, threads, 0, stream>>>(ix, norms);
+        norms_kernel<cos_half_t<bf16_conv_t>><<<(ix.n + threads - 1) / threads, threads, 0, stream>>>(ix, norms, slots);
     } else
         return cudaErrorInvalidValue;
     return cudaGetLastError();
@@ -1193,9 +1196,10 @@ cudaError_t search_compute_norms(device_index_t const& ix, float* norms, cudaStr
 
 /* ---- the int8 shadow of cos / ip f32 rows (prefilter_bound.h): one warp per row -------------------------- */
 
-__global__ void shadow_kernel(device_index_t ix, float const* norms, int8_t* codes, pf_record_t* records) {
-    uint32_t const lane = threadIdx.x & 31, row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (row >= ix.n) return; /* uniform per warp */
+__global__ void shadow_kernel(device_index_t ix, float const* norms, int8_t* codes, pf_record_t* records, uint32_t const* slots) {
+    uint32_t const lane = threadIdx.x & 31, i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= ix.n) return; /* uniform per warp */
+    uint32_t const row = slots ? slots[i] : i;
     float const* b = reinterpret_cast<float const*>(ix.vectors + (size_t)row * ix.vec_stride);
     double mx = 0.0;
     bool finite = true;
@@ -1237,10 +1241,10 @@ bool search_needs_shadow(device_index_t const& ix) {
 uint32_t search_code_stride(device_index_t const& ix) { return (ix.dims + 15u) & ~15u; }
 
 cudaError_t search_compute_shadow(device_index_t const& ix, float const* norms, int8_t* codes, pf_record_t* records,
-                                  cudaStream_t stream) {
+                                  cudaStream_t stream, uint32_t const* slots) {
     if (!ix.n) return cudaSuccess;
     uint32_t const rows_per_block = 8;
-    shadow_kernel<<<(ix.n + rows_per_block - 1) / rows_per_block, 32 * rows_per_block, 0, stream>>>(ix, norms, codes, records);
+    shadow_kernel<<<(ix.n + rows_per_block - 1) / rows_per_block, 32 * rows_per_block, 0, stream>>>(ix, norms, codes, records, slots);
     return cudaGetLastError();
 }
 

@@ -54,7 +54,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_shards_unique_id", "usearch_b200_shards_join", "usearch_b200_sharded_search_many",
     "usearch_b200_sharded_search_many_device", "usearch_b200_shards_payload_bytes", "usearch_b200_merge_topk",
     "usearch_b200_search_many_enqueue", "usearch_b200_search_many_finish", "usearch_b200_tune",
-    "usearch_b200_launch_plan",
+    "usearch_b200_launch_plan", "usearch_b200_remove_many", "usearch_b200_count_many", "usearch_b200_change_reuse_removed",
+    "usearch_b200_reuse_removed",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -146,6 +147,13 @@ def load_library() -> C.CDLL:
     lib.usearch_get.argtypes = [C.c_void_p, C.c_uint64, C.c_size_t, C.c_void_p, C.c_int, err]
     lib.usearch_remove.restype = C.c_size_t
     lib.usearch_remove.argtypes = [C.c_void_p, C.c_uint64, err]
+    lib.usearch_b200_remove_many.restype = C.c_size_t
+    lib.usearch_b200_remove_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_bool, C.POINTER(C.c_size_t), err]
+    lib.usearch_b200_count_many.restype = C.c_size_t
+    lib.usearch_b200_count_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, err]
+    lib.usearch_b200_change_reuse_removed.argtypes = [C.c_void_p, C.c_bool, err]
+    lib.usearch_b200_reuse_removed.restype = C.c_bool
+    lib.usearch_b200_reuse_removed.argtypes = [C.c_void_p]
     lib.usearch_rename.restype = C.c_size_t
     lib.usearch_rename.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, err]
     lib.usearch_b200_shards_unique_id.argtypes = [C.c_void_p, err]
@@ -238,6 +246,7 @@ class Index:
         self._dtype = dtype
         self._expansion_search = expansion_search
         self._keepalive = None
+        self.last_pruned_edges = 0  # links erased by the last remove(..., compact=True)
         if path is not None:
             (self.view if view else self.load)(path)
 
@@ -367,13 +376,27 @@ class Index:
                                                SCALAR_KIND[kind or self._dtype], C.byref(err))
         _raise(err)
 
-    def contains(self, key: int) -> bool:
-        return bool(self._lib.usearch_contains(self._h, int(key), None))
+    def _count_many(self, keys) -> np.ndarray:
+        keys = np.ascontiguousarray(np.fromiter(keys, dtype=np.uint64) if not isinstance(keys, np.ndarray) else keys,
+                                    dtype=np.uint64)
+        counts = np.zeros(keys.shape[0], dtype=np.uintp)
+        self._lib.usearch_b200_count_many(self._h, keys.ctypes.data_as(C.c_void_p), keys.shape[0],
+                                          counts.ctypes.data_as(C.c_void_p), None)
+        return counts
+
+    def contains(self, keys) -> Union[bool, np.ndarray]:
+        """One key -> bool; an iterable of keys -> a bool array."""
+        if np.isscalar(keys) or isinstance(keys, int):
+            return bool(self._lib.usearch_contains(self._h, int(keys), None))
+        return self._count_many(keys) > 0
 
     __contains__ = contains
 
-    def count(self, key: int) -> int:
-        return int(self._lib.usearch_count(self._h, int(key), None))
+    def count(self, keys) -> Union[int, np.ndarray]:
+        """One key -> the entries stored under it; an iterable of keys -> an array of counts."""
+        if np.isscalar(keys) or isinstance(keys, int):
+            return int(self._lib.usearch_count(self._h, int(keys), None))
+        return self._count_many(keys).astype(np.uint64)
 
     def get(self, key: int, dtype: Optional[str] = None, count: int = 1) -> Optional[np.ndarray]:
         """`Index.get` (index.py:820-870): the vector(s) stored under `key`, or None."""
@@ -388,11 +411,32 @@ class Index:
             return None
         return out[0] if count == 1 else out[:found]
 
-    def remove(self, key: int) -> int:
+    def remove(self, keys, *, compact: bool = False, threads: int = 0) -> int:
+        """`Index.remove` (python/lib.cpp:1192-1227): one key or an iterable of keys; returns the number of entries
+        removed. Their slots wait for reuse (see `reuse_removed`). With `compact`, every link that leads to a removed
+        entry is erased on the GPU; `last_pruned_edges` then holds how many. `threads` is accepted for compatibility."""
+        del threads
+        if np.isscalar(keys) or isinstance(keys, int):
+            keys = np.array([int(keys)], dtype=np.uint64)
+        else:
+            keys = np.ascontiguousarray(np.fromiter(keys, dtype=np.uint64) if not isinstance(keys, np.ndarray) else keys,
+                                        dtype=np.uint64)
         err = C.c_char_p()
-        n = self._lib.usearch_remove(self._h, int(key), C.byref(err))
+        pruned = C.c_size_t(0)
+        n = self._lib.usearch_b200_remove_many(self._h, keys.ctypes.data_as(C.c_void_p), keys.shape[0], bool(compact),
+                                               C.byref(pruned), C.byref(err))
         _raise(err)
+        self.last_pruned_edges = int(pruned.value)
         return int(n)
+
+    @property
+    def reuse_removed(self) -> bool:
+        """Whether `add` puts new entries into the slots of removed ones (oldest first) before appending. Off by default."""
+        return bool(self._lib.usearch_b200_reuse_removed(self._h))
+
+    @reuse_removed.setter
+    def reuse_removed(self, on: bool) -> None:
+        self._lib.usearch_b200_change_reuse_removed(self._h, bool(on), None)
 
     def rename(self, key_from: int, key_to: int) -> int:
         err = C.c_char_p()
