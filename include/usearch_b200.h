@@ -186,6 +186,29 @@ size_t usearch_b200_count_many(usearch_index_t index, usearch_key_t const* keys,
 void usearch_b200_change_reuse_removed(usearch_index_t index, bool reuse, usearch_error_t* error);
 bool usearch_b200_reuse_removed(usearch_index_t index);
 
+/* NEW (additive). Semantic join (index_dense_gt::join, index_dense.hpp:1762-1786; stable marriages, index.hpp:4345-4543) of
+ * `a` with `b`, with the decisions of the reference's run on one thread. The side with fewer slots (removed entries
+ * count) proposes; proposals are searches of the other index (approximate, or brute force with `exact`) with expansion
+ * max(expansion_search(a), expansion_search(b)). `max_proposals` 0 means log(men) + 1, clamped to the men; at most 65535.
+ * Removed entries take part, as in the reference, and are exported under the free key, so the number of pairs can exceed
+ * usearch_size. Writes the engaged pairs (a key, b key) in the reference's export order into `a_keys_out` /
+ * `b_keys_out`, each holding `capacity` keys; min(usearch_capacity(a), usearch_capacity(b)) is always enough. Returns the
+ * number of pairs, or 0 and an error when they do not fit. `stats4_out` (may be NULL) receives intersection_size,
+ * engagements, visited_members and computed_distances. Both handles must be on one device, not sharded, and share metric,
+ * scalar kind and dimensions. */
+size_t usearch_b200_join(usearch_index_t a, usearch_index_t b, size_t max_proposals, bool exact, usearch_key_t* a_keys_out,
+                         usearch_key_t* b_keys_out, size_t capacity, size_t* stats4_out, usearch_error_t* error);
+/* NEW (additive). Wall-clock milliseconds of the last usearch_b200_join called with `index` as `a`: proposal searches
+ * (launches and copies back), pair distances, and the host replay without the columns it waited for. */
+void usearch_b200_last_join_ms(usearch_index_t index, float* out3);
+/* NEW (additive). out[i] = the distance between the vectors stored under left_keys[i] and right_keys[i], FLT_MAX where a
+ * key is missing, one GPU launch. With one vector per key this is distance_between(left, right).min
+ * (index_dense.hpp:808-862) bit for bit. A multi index takes the minimum over EVERY pair of their vectors; the reference
+ * pairs only the first vector under the left key with each vector under the right key (its loop does not rewind the
+ * right range), so the two differ when the left key holds several vectors. */
+void usearch_b200_pairwise_distances(usearch_index_t index, usearch_key_t const* left_keys, usearch_key_t const* right_keys, size_t n,
+                                     usearch_distance_t* out, usearch_error_t* error);
+
 /* ---- additive: sharded search, one process per GPU (SURVEY.md §8e) ------------------------------------------------ */
 
 /* The reference's `Indexes` (python/lib.cpp:74-107, :321-402) searches every query in every shard and merges by distance. Here

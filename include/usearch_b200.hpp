@@ -315,6 +315,39 @@ class index_dense_t {
         for (std::size_t i = 0; i != queries; ++i) batch.computed_distances += computed[i], batch.visited_members += visited[i];
         return batch;
     }
+
+    /* join_result_t (index.hpp:1577-1590) and index_dense_gt::join (index_dense.hpp:1762-1786): every engaged pair is
+     * written as man_to_woman[key of this] = key of women, woman_to_man[key of women] = key of this, in the reference's
+     * export order, into any map-like pair of outputs (`operator[]` on keys). The one-thread run of the reference. */
+    struct join_result_t {
+        error_t error{};
+        std::size_t intersection_size = 0;
+        std::size_t engagements = 0;
+        std::size_t visited_members = 0;
+        std::size_t computed_distances = 0;
+        explicit operator bool() const noexcept { return !error; }
+    };
+    template <typename man_to_woman_at, typename woman_to_man_at>
+    join_result_t join(index_dense_t const& women, std::size_t max_proposals, bool exact, man_to_woman_at&& man_to_woman,
+                       woman_to_man_at&& woman_to_man) const {
+        join_result_t result;
+        std::size_t const slots = capacity() < women.capacity() ? capacity() : women.capacity();
+        std::vector<vector_key_t> a(slots), b(slots);
+        std::size_t stats[4] = {0, 0, 0, 0};
+        usearch_error_t error = nullptr;
+        std::size_t const pairs = usearch_b200_join(handle_, women.handle_, max_proposals, exact, a.data(), b.data(), slots, stats, &error);
+        result.error = error;
+        if (error) return result;
+        for (std::size_t i = 0; i != pairs; ++i) {
+            man_to_woman[a[i]] = b[i];
+            woman_to_man[b[i]] = a[i];
+        }
+        result.intersection_size = stats[0];
+        result.engagements = stats[1];
+        result.visited_members = stats[2];
+        result.computed_distances = stats[3];
+        return result;
+    }
 };
 
 struct index_dense_state_result_t {

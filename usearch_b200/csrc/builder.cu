@@ -34,6 +34,7 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "cuda_check.h"
 #include "frozen_index.h"
 #include "metrics.cuh"
 #include "warp_primitives.cuh"
@@ -46,18 +47,6 @@ constexpr int LINK_THREADS = 256;         /* 8 warps work on one refine */
 constexpr uint32_t LINK_CAND_MAX = 256;   /* candidates one refine can hold (expansion_add and list + arrivals are cut to it) */
 constexpr int LINK_LOADS_IN_FLIGHT = 8;
 
-char const* cuda_error(cudaError_t e) {
-    if (e == cudaSuccess) return nullptr;
-    cudaGetLastError();
-    if (e == cudaErrorMemoryAllocation) return "Out of GPU memory!";
-    static thread_local char message[160];
-    std::snprintf(message, sizeof(message), "CUDA failure: %s", cudaGetErrorString(e));
-    return message;
-}
-#define CU(call)                                                \
-    do {                                                        \
-        if (char const* err_ = cuda_error((call))) return err_; \
-    } while (0)
 
 uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
@@ -435,6 +424,47 @@ cudaError_t launch_pair(device_index_t const& ix, uint8_t const* query, float* o
     BUILD_DISPATCH(launch_pair_t, ix, query, out, s)
 }
 
+/* ---- gathered pairs: metric(a.rows[slot_a[j]], b.rows[slot_b[j]]) for join and pairwise_distance ----------------- */
+
+/* One warp per pair, every lane group of LPV lanes walking both rows as pair_distance_kernel does (the groups of a warp
+ * compute the same value, so `prepare` can use the whole warp). cos takes the stored norms of both rows where the index
+ * keeps them: the same chain as `prepare`, so the bits equal usearch_distance for the same two vectors. */
+template <class M>
+__global__ void pair_distances_kernel(device_index_t const a, device_index_t const b, uint32_t const* slot_a,
+                                      uint32_t const* slot_b, uint32_t n, float* out) {
+    constexpr int LPV = M::LPV;
+    int const lane = threadIdx.x & 31, sub = lane % LPV;
+    uint32_t const warps = gridDim.x * (blockDim.x >> 5);
+    for (uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += warps) {
+        uint32_t const sa = slot_a[j], sb = slot_b[j];
+        uint4 const* qa = reinterpret_cast<uint4 const*>(a.vectors + (size_t)sa * a.vec_stride);
+        uint4 const* vb = reinterpret_cast<uint4 const*>(b.vectors + (size_t)sb * b.vec_stride);
+        typename M::qconst_t qc;
+        if constexpr (M::NORMS) {
+            if (a.norms) qc.a2 = __ldg(a.norms + sa);
+            else qc = M::prepare(qa, a.chunks16, lane);
+        } else
+            qc = M::prepare(qa, a.chunks16, lane);
+        typename M::acc_t acc;
+        M::init(acc);
+        for (uint32_t c = sub; c < a.chunks16; c += LPV) M::step(acc, __ldg(vb + c), __ldg(qa + c));
+        float d = M::finish(acc, qc);
+        if constexpr (M::NORMS) d = M::finalize(d, qc, b.norms ? __ldg(b.norms + sb) : M::prepare(vb, b.chunks16, lane).a2);
+        if (lane == 0) out[j] = d;
+    }
+}
+template <class M>
+cudaError_t launch_pairs_t(device_index_t const& ix, device_index_t const& b, uint32_t const* slot_a, uint32_t const* slot_b,
+                           uint32_t n, float* out, cudaStream_t s) {
+    unsigned const blocks = (unsigned)std::min<uint32_t>((n + 7) / 8, 65535u * 4);
+    pair_distances_kernel<M><<<blocks, 256, 0, s>>>(ix, b, slot_a, slot_b, n, out);
+    return cudaGetLastError();
+}
+cudaError_t launch_pairs(device_index_t const& ix, device_index_t const& b, uint32_t const* slot_a, uint32_t const* slot_b,
+                         uint32_t n, float* out, cudaStream_t s) {
+    BUILD_DISPATCH(launch_pairs_t, ix, b, slot_a, slot_b, n, out, s)
+}
+
 /* ---- scalar casts on the device (index_plugins.hpp:1105-1224) --------------------------------------------------------- */
 
 __device__ __forceinline__ uint16_t f32_to_bf16_bits(float f) { /* simsimd_f32_to_bf16: round to nearest even, quiet NaNs */
@@ -595,6 +625,26 @@ char const* pair_distance_device(device_index_t const& shape, uint8_t const* d_a
     ix.vectors = d_b;
     ix.n = 1;
     CU(launch_pair(ix, d_a, d_out, s));
+    return nullptr;
+}
+
+/* metric(a.rows[slot_a[j]], b.rows[slot_b[j]]) for j < n; a and b share metric, scalar kind and dimensions */
+char const* pair_distances_device(device_index_t const& a, device_index_t const& b, uint32_t const* d_slot_a, uint32_t const* d_slot_b,
+                                  size_t n, float* d_out, cudaStream_t s) {
+    if (!n) return nullptr;
+    if (n > 0xFFFFFFFFull) return "Too many pairs in one batch";
+    CU(launch_pairs(a, b, d_slot_a, d_slot_b, (uint32_t)n, d_out, s));
+    return nullptr;
+}
+
+__global__ void iota_u64_kernel(uint64_t* out, uint32_t n) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = i;
+}
+
+char const* iota_u64_device(uint64_t* d_out, size_t n, cudaStream_t s) {
+    if (!n) return nullptr;
+    iota_u64_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 65535), 256, 0, s>>>(d_out, (uint32_t)n);
+    CU(cudaGetLastError());
     return nullptr;
 }
 

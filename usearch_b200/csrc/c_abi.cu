@@ -242,7 +242,11 @@ void usearch_reserve(usearch_index_t index, size_t capacity, usearch_error_t* er
 size_t usearch_expansion_add(usearch_index_t index, usearch_error_t*) { return as_index(index)->expansion_add; }
 size_t usearch_expansion_search(usearch_index_t index, usearch_error_t*) { return as_index(index)->expansion_search; }
 void usearch_change_expansion_add(usearch_index_t index, size_t expansion, usearch_error_t*) { as_index(index)->expansion_add = expansion; }
-void usearch_change_expansion_search(usearch_index_t index, size_t expansion, usearch_error_t*) { as_index(index)->expansion_search = expansion; }
+void usearch_change_expansion_search(usearch_index_t index, size_t expansion, usearch_error_t*) {
+    /* under the lock: a join reads and temporarily replaces it for the whole call */
+    std::lock_guard<std::mutex> lock(as_index(index)->mutex);
+    as_index(index)->expansion_search = expansion;
+}
 void usearch_change_threads_add(usearch_index_t, size_t, usearch_error_t*) {}
 void usearch_change_threads_search(usearch_index_t, size_t, usearch_error_t*) {}
 
@@ -466,6 +470,28 @@ void usearch_b200_change_reuse_removed(usearch_index_t index, bool reuse, usearc
 }
 
 bool usearch_b200_reuse_removed(usearch_index_t index) { return as_index(index)->reuse_removed; }
+
+size_t usearch_b200_join(usearch_index_t a, usearch_index_t b, size_t max_proposals, bool exact, usearch_key_t* a_keys_out,
+                         usearch_key_t* b_keys_out, size_t capacity, size_t* stats4_out, usearch_error_t* error) {
+    std::vector<uint64_t> ak, bk;
+    size_t stats[4] = {0, 0, 0, 0};
+    char const* e = guarded([&] { return as_index(a)->join(*as_index(b), max_proposals, exact, ak, bk, stats); });
+    if (e) { set_error(error, e); return 0; }
+    if (ak.size() > capacity) { set_error(error, "Output arrays too small for the engaged pairs: size them to min(capacity(a), capacity(b))"); return 0; }
+    if (!ak.empty()) {
+        std::memcpy(a_keys_out, ak.data(), ak.size() * sizeof(uint64_t));
+        std::memcpy(b_keys_out, bk.data(), bk.size() * sizeof(uint64_t));
+    }
+    if (stats4_out) std::memcpy(stats4_out, stats, sizeof(stats));
+    return ak.size();
+}
+
+void usearch_b200_last_join_ms(usearch_index_t index, float* out3) { std::memcpy(out3, as_index(index)->last_join_ms, 3 * sizeof(float)); }
+
+void usearch_b200_pairwise_distances(usearch_index_t index, usearch_key_t const* left_keys, usearch_key_t const* right_keys, size_t n,
+                                     usearch_distance_t* out, usearch_error_t* error) {
+    set_error(error, guarded([&] { return as_index(index)->pairwise_distances(left_keys, right_keys, n, out); }));
+}
 
 size_t usearch_rename(usearch_index_t index, usearch_key_t from, usearch_key_t to, usearch_error_t* error) { /* c/lib.cpp:448-455 */
     frozen_index_t* ix = as_index(index);

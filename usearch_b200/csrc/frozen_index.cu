@@ -10,6 +10,7 @@
  *    index.hpp:3016-3075        expansion = max(config.expansion or 64, wanted)
  *    index_plugins.hpp:1105-1224 query casts
  */
+#include "cuda_check.h"
 #include "frozen_index.h"
 #include "prefilter_bound.h"
 
@@ -28,19 +29,6 @@ int16_t rd_i16(uint8_t const* p) { int16_t v; std::memcpy(&v, p, 2); return v; }
 uint32_t ceil2(uint64_t v) { uint64_t r = 1; while (r < v) r <<= 1; return (uint32_t)std::min<uint64_t>(r, 1ull << 31); }
 uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
-char const* cuda_error(cudaError_t e) {
-    if (e == cudaSuccess) return nullptr;
-    cudaGetLastError();
-    if (e == cudaErrorMemoryAllocation) return "Out of GPU memory!";
-    static thread_local char message[160];
-    std::snprintf(message, sizeof(message), "CUDA failure: %s", cudaGetErrorString(e));
-    return message;
-}
-
-#define CU(call)                                             \
-    do {                                                     \
-        if (char const* err_ = cuda_error((call))) return err_; \
-    } while (0)
 
 } // namespace
 

@@ -223,6 +223,14 @@ struct frozen_index_t {
     char const* rename_key(uint64_t from, uint64_t to, size_t* renamed);
     char const* get_vectors(uint64_t key, size_t max_count, void* out, uint32_t out_scalar, size_t* found);
 
+    /* join.cu: the reference's stable-marriage `join` of this index (a) with `other` (b), replayed as its one-thread run.
+     * Pairs (a key, b key) come out in the reference's export order; stats as join_result_t. */
+    char const* join(frozen_index_t& other, size_t max_proposals, bool exact, std::vector<uint64_t>& a_keys,
+                     std::vector<uint64_t>& b_keys, size_t stats[4]);
+    float last_join_ms[3] = {0.f, 0.f, 0.f}; /* wall clock of the last join called on this handle: search | pairs | replay */
+    /* distance_between(left[i], right[i]).min for every i; a missing key gives FLT_MAX */
+    char const* pairwise_distances(uint64_t const* left, uint64_t const* right, size_t n, float* out);
+
     /* sharded search (shards.cu): this handle is shard `rank` of `world`, one process per GPU */
     shard_group_t* shards = nullptr;
     char const* join_shards(int rank, int world, void const* unique_id128);
@@ -282,6 +290,10 @@ char const* shards_merge_host(void const* payloads, int world, size_t nq, size_t
 char const* cast_rows_device(uint8_t const* src, size_t src_stride, uint32_t from, uint8_t* dst, size_t dst_stride, uint32_t to,
                              size_t dims, size_t rows, cudaStream_t stream);
 char const* pair_distance_device(device_index_t const& shape, uint8_t const* d_a, uint8_t const* d_b, float* d_out, cudaStream_t stream);
+/* metric(a.rows[slot_a[j]], b.rows[slot_b[j]]) for j < n, one launch; a and b share metric, scalar kind and dimensions */
+char const* pair_distances_device(device_index_t const& a, device_index_t const& b, uint32_t const* d_slot_a, uint32_t const* d_slot_b,
+                                  size_t n, float* d_out, cudaStream_t stream);
+char const* iota_u64_device(uint64_t* d_out, size_t n, cudaStream_t stream);
 
 char const* pair_distance_host(void const* a, void const* b, uint32_t scalar, size_t dimensions, uint32_t metric, float* result);
 int default_device(); /* USEARCH_B200_DEVICE, else LOCAL_RANK (one process per GPU under torchrun), else 0 */

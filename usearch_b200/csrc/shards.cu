@@ -17,24 +17,13 @@
 
 #include <cstring>
 
+#include "cuda_check.h"
 #include "frozen_index.h"
 
 namespace usearch_b200 {
 
 namespace {
 
-char const* cuda_error(cudaError_t e) {
-    if (e == cudaSuccess) return nullptr;
-    cudaGetLastError();
-    if (e == cudaErrorMemoryAllocation) return "Out of GPU memory!";
-    static thread_local char message[160];
-    std::snprintf(message, sizeof(message), "CUDA failure: %s", cudaGetErrorString(e));
-    return message;
-}
-#define CU(call)                                                \
-    do {                                                        \
-        if (char const* err_ = cuda_error((call))) return err_; \
-    } while (0)
 
 /* ---- the five NCCL entry points this file needs, resolved at run time (nccl.h: ncclResult_t == int, 0 = success) ---- */
 

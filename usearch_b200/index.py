@@ -12,7 +12,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 from dataclasses import dataclass
-from typing import Optional, Union
+from typing import Dict, Optional, Union
 
 import numpy as np
 
@@ -55,7 +55,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_sharded_search_many_device", "usearch_b200_shards_payload_bytes", "usearch_b200_merge_topk",
     "usearch_b200_search_many_enqueue", "usearch_b200_search_many_finish", "usearch_b200_tune",
     "usearch_b200_launch_plan", "usearch_b200_remove_many", "usearch_b200_count_many", "usearch_b200_change_reuse_removed",
-    "usearch_b200_reuse_removed",
+    "usearch_b200_reuse_removed", "usearch_b200_join", "usearch_b200_pairwise_distances",
+    "usearch_b200_last_join_ms",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -154,6 +155,11 @@ def load_library() -> C.CDLL:
     lib.usearch_b200_change_reuse_removed.argtypes = [C.c_void_p, C.c_bool, err]
     lib.usearch_b200_reuse_removed.restype = C.c_bool
     lib.usearch_b200_reuse_removed.argtypes = [C.c_void_p]
+    lib.usearch_b200_join.restype = C.c_size_t
+    lib.usearch_b200_join.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_bool, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                      err]
+    lib.usearch_b200_last_join_ms.argtypes = [C.c_void_p, C.c_void_p]
+    lib.usearch_b200_pairwise_distances.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, err]
     lib.usearch_rename.restype = C.c_size_t
     lib.usearch_rename.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, err]
     lib.usearch_b200_shards_unique_id.argtypes = [C.c_void_p, err]
@@ -247,6 +253,8 @@ class Index:
         self._expansion_search = expansion_search
         self._keepalive = None
         self.last_pruned_edges = 0  # links erased by the last remove(..., compact=True)
+        self.last_join_stats = {}  # intersection_size, engagements, visited_members, computed_distances of the last join
+        self.last_join_ms = {}  # its wall clock per phase: search, pair_distances, replay
         if path is not None:
             (self.view if view else self.load)(path)
 
@@ -446,6 +454,55 @@ class Index:
 
     def clear(self) -> None:
         self._lib.usearch_clear(self._h, None)
+
+    # ---- join and pairwise distances (index.py:1170-1200, :1263-1283) -------------------------------------------
+    def join(self, other: "Index", max_proposals: int = 0, exact: bool = False, progress=None) -> Dict[int, int]:
+        """`Index.join`: a one-to-one "semantic join" of `self` with `other` by stable marriages. Returns a mapping from
+        keys of `self` to keys of `other`. The smaller index proposes, each proposal a search of the other one (`exact`:
+        brute force); the searches run as batched GPU launches and the proposals are then replayed as the reference's
+        single-threaded run makes them, so the result is deterministic.
+
+        `max_proposals=0` means log(n) + 1 for the proposing side's size n. The reference's Python `join` adds its thread
+        count instead of 1, so pass `max_proposals` explicitly to reproduce a multi-threaded reference run's budget.
+        `progress` is accepted for compatibility and ignored. The four counters of the run go to `last_join_stats`, the
+        wall-clock milliseconds of its three phases (proposal searches, pair distances, host replay) to `last_join_ms`."""
+        del progress
+        n = min(self.capacity, other.capacity)  # >= the slots of either side, removed entries included
+        a_keys = np.zeros(max(n, 1), dtype=np.uint64)
+        b_keys = np.zeros(max(n, 1), dtype=np.uint64)
+        stats = np.zeros(4, dtype=np.uintp)
+        err = C.c_char_p()
+        found = self._lib.usearch_b200_join(self._h, other._h, int(max_proposals), bool(exact), a_keys.ctypes.data_as(C.c_void_p),
+                                            b_keys.ctypes.data_as(C.c_void_p), a_keys.shape[0], stats.ctypes.data_as(C.c_void_p),
+                                            C.byref(err))
+        _raise(err)
+        self.last_join_stats = dict(zip(("intersection_size", "engagements", "visited_members", "computed_distances"),
+                                        (int(x) for x in stats)))
+        ms = np.zeros(3, dtype=np.float32)
+        self._lib.usearch_b200_last_join_ms(self._h, ms.ctypes.data_as(C.c_void_p))
+        self.last_join_ms = dict(zip(("search", "pair_distances", "replay"), (float(x) for x in ms)))
+        # in export order: on a repeated key (a multi index) the last pair wins, as in the reference
+        return dict(zip(a_keys[:found].tolist(), b_keys[:found].tolist()))
+
+    def pairwise_distance(self, left, right) -> Union[np.ndarray, float]:
+        """`Index.pairwise_distance`: the distance between the vectors stored under two keys, or between the keys of
+        two equally long arrays element by element; where a key is missing, the largest finite float. With one vector per
+        key this is the reference's `distance_between(left, right).min`. Where keys hold several vectors (multi index) it
+        is the minimum over every pair, a documented difference: the reference pairs only the first vector under `left`
+        with each vector under `right`."""
+        single = np.isscalar(left) or isinstance(left, int)
+        if single != (np.isscalar(right) or isinstance(right, int)):
+            raise ValueError("Pass two keys or two arrays of keys")
+        left = np.ascontiguousarray(np.atleast_1d(np.asarray(left)), dtype=np.uint64)
+        right = np.ascontiguousarray(np.atleast_1d(np.asarray(right)), dtype=np.uint64)
+        if left.shape != right.shape:
+            raise ValueError("The two key arrays must have the same length")
+        out = np.zeros(left.shape[0], dtype=np.float32)
+        err = C.c_char_p()
+        self._lib.usearch_b200_pairwise_distances(self._h, left.ctypes.data_as(C.c_void_p), right.ctypes.data_as(C.c_void_p),
+                                                  left.shape[0], out.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        return float(out[0]) if single else out
 
     # ---- search (index.py:700-748) ---------------------------------------------------------------
     def _kind_of(self, vectors: np.ndarray) -> str:
