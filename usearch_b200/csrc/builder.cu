@@ -349,6 +349,11 @@ __global__ void __launch_bounds__(LINK_THREADS, 3) link_reverse_kernel(__grid_co
         if (ix.metric == METRIC_IP) return FN<ip_f32_t>(__VA_ARGS__);                               \
         if (ix.metric == METRIC_COS) return FN<cos_f32_t>(__VA_ARGS__);                             \
         break;                                                                                      \
+    case SCALAR_F64:                                                                                \
+        if (ix.metric == METRIC_L2SQ) return FN<l2sq_f64_t>(__VA_ARGS__);                           \
+        if (ix.metric == METRIC_IP) return FN<ip_f64_t>(__VA_ARGS__);                               \
+        if (ix.metric == METRIC_COS) return FN<cos_f64_t>(__VA_ARGS__);                             \
+        break;                                                                                      \
     case SCALAR_F16:                                                                                \
         if (ix.metric == METRIC_L2SQ) return FN<l2sq_half_t<f16_conv_t>>(__VA_ARGS__);              \
         if (ix.metric == METRIC_IP) return FN<ip_half_t<f16_conv_t>>(__VA_ARGS__);                  \
@@ -532,6 +537,19 @@ __global__ void cast_rows_to_i8_kernel(uint8_t const* src, size_t src_stride, ui
     }
 }
 
+/* cast_gt<*, f64> (index_plugins.hpp:1105-1224), one thread per element: f32, f16 and bf16 widen exactly, b1 gives 1.0 or
+ * 0.0, and i8 is cast_from_i8_gt<f64>, a double division `(double)x / 127.0` (not the f32 quotient of load_scalar) */
+__global__ void cast_elements_to_f64_kernel(uint8_t const* src, size_t src_stride, uint32_t from, uint8_t* dst, size_t dst_stride,
+                                            uint32_t dims, size_t rows) {
+    size_t const gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= rows * dims) return;
+    size_t const r = gid / dims;
+    uint32_t const i = (uint32_t)(gid - r * dims);
+    uint8_t const* in = src + r * src_stride;
+    double const v = from == SCALAR_I8 ? __ddiv_rn((double)reinterpret_cast<int8_t const*>(in)[i], 127.0) : load_scalar(in, from, i);
+    reinterpret_cast<double*>(dst + r * dst_stride)[i] = v;
+}
+
 /* ---- removal and reuse: per-slot edits of `keys` / `deleted_bits`, rows scattered into reused slots ------------------ */
 
 /* new_keys == NULL: index_dense_gt::remove (index_dense.hpp:1479-1513), the slot takes the free key and its deleted bit;
@@ -610,6 +628,8 @@ char const* cast_rows_device(uint8_t const* src, size_t src_stride, uint32_t fro
     if (!bits_per_scalar(from)) return "Unknown scalar kind!";
     if (to == SCALAR_I8) {
         cast_rows_to_i8_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, s>>>(src, src_stride, from, dst, dst_stride, (uint32_t)dims, rows);
+    } else if (to == SCALAR_F64) {
+        cast_elements_to_f64_kernel<<<(unsigned)((rows * dims + 255) / 256), 256, 0, s>>>(src, src_stride, from, dst, dst_stride, (uint32_t)dims, rows);
     } else if (to == SCALAR_F32 || to == SCALAR_F16 || to == SCALAR_BF16 || to == SCALAR_B1) {
         size_t const total = rows * (to == SCALAR_B1 ? (dims + 7) / 8 : dims);
         cast_elements_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(src, src_stride, from, dst, dst_stride, to, (uint32_t)dims, rows);

@@ -508,6 +508,11 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
         else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_f32_t>(tiled, ix, a, swap, grid, smem, stream);
         else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_f32_t>(tiled, ix, a, swap, grid, smem, stream);
         break;
+    case SCALAR_F64:
+        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_f64_t>(tiled, ix, a, swap, grid, smem, stream);
+        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_f64_t>(tiled, ix, a, swap, grid, smem, stream);
+        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_f64_t>(tiled, ix, a, swap, grid, smem, stream);
+        break;
     case SCALAR_F16:
         if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_half_t<f16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
         else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_half_t<f16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);

@@ -11,6 +11,7 @@
  *    index_plugins.hpp:1105-1224 query casts
  */
 #include "cuda_check.h"
+#include "f64_casts.h"
 #include "frozen_index.h"
 #include "prefilter_bound.h"
 
@@ -1119,6 +1120,15 @@ float half_bits_to_f32(uint16_t h) {
 char const* cast_stored_row(uint32_t from, uint32_t to, size_t dims, uint8_t const* src, uint8_t* dst) {
     size_t const to_bytes = (dims * bits_per_scalar(to) + 7) / 8;
     if (from == to) { std::memcpy(dst, src, to_bytes); return nullptr; }
+    if (from == SCALAR_F64) { /* cast_gt<f64, *>: i8 and b1 read the doubles, the rest narrow to f32 first */
+        std::vector<double> x(dims);
+        std::memcpy(x.data(), src, dims * 8);
+        if (to == SCALAR_I8) { cast_f64_to_i8(x.data(), dims, reinterpret_cast<int8_t*>(dst)); return nullptr; }
+        if (to == SCALAR_B1) { cast_f64_to_b1(x.data(), dims, dst); return nullptr; }
+        std::vector<float> row(dims);
+        for (size_t j = 0; j < dims; ++j) row[j] = (float)x[j];
+        return cast_queries(SCALAR_F32, to, dims, reinterpret_cast<uint8_t const*>(row.data()), dims * 4, 1, dst, to_bytes);
+    }
     std::vector<float> row(dims);
     for (size_t j = 0; j < dims; ++j) {
         switch (from) {

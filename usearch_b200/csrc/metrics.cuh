@@ -18,6 +18,8 @@
  *           SimSIMD's zero rules and clamp (spatial.h:1544-1585 uses rsqrt14+Newton, which differs
  *           by <= 1 ULP(f32) and cannot be reproduced off-x86; see oracle/metrics_pinned.h).
  *    ip   : 1.0f - dot in f32 (index_plugins.hpp:1914-1916: the f64 result is cast to f32 first).
+ *    f64  : 8 accumulators, element i -> accumulator i mod 8; lane `sub` owns accumulators 2 sub, 2 sub + 1
+ *           (spatial.h:1622-1674, dot.h:1320-1341), see the f64 section below.
  *    i8   : exact i32 sums via dp4a (dot.h:1749-1775, spatial.h:1880-1972).
  *    b1   : exact popcounts (binary.h:92-105, :271-347).
  */
@@ -170,6 +172,110 @@ struct cos_f32_t {
     }
     static __device__ __forceinline__ qconst_t prepare(uint4 const* q4, uint32_t chunks16, int lane) {
         return {self_dot(q4, chunks16, lane)};
+    }
+};
+
+/* ---- f64 -------------------------------------------------------------------------------- */
+/*
+ *  simsimd_{l2sq,dot,cos}_f64_skylake (spatial.h:1622-1674, dot.h:1320-1341): 8 f64 accumulators, element i ->
+ *  accumulator i mod 8, one fma per element, then _mm512_reduce_add_pd, which GCC's avx512fintrin.h evaluates as
+ *  ((v0+v4)+(v2+v6)) + ((v1+v5)+(v3+v7)). A 16-byte chunk j holds elements 2j and 2j+1, i.e. accumulators
+ *  2(j mod 4) and 2(j mod 4)+1, so FOUR lanes share a vector as for f32: lane `sub` owns chunks sub, sub+4, ... and
+ *  accumulators 2 sub and 2 sub + 1. The tree is the one of reduce_words_f64 without the widening from f32.
+ *  The f64 rows have no stored norm (`norms` is f32): cos accumulates b2 in the loop, like cos_i8_t.
+ */
+__device__ __forceinline__ double reduce8_lanes_f64(double a, double b) {
+    a = __dadd_rn(a, __shfl_xor_sync(0xffffffffu, a, 2)); /* lanes 0,2: v0+v4 | lanes 1,3: v2+v6 */
+    b = __dadd_rn(b, __shfl_xor_sync(0xffffffffu, b, 2)); /* lanes 0,2: v1+v5 | lanes 1,3: v3+v7 */
+    a = __dadd_rn(a, __shfl_xor_sync(0xffffffffu, a, 1)); /* (v0+v4)+(v2+v6) */
+    b = __dadd_rn(b, __shfl_xor_sync(0xffffffffu, b, 1)); /* (v1+v5)+(v3+v7) */
+    return __dadd_rn(a, b);
+}
+
+__device__ __forceinline__ double lo_f64(uint4 x) { return __hiloint2double((int)x.y, (int)x.x); }
+__device__ __forceinline__ double hi_f64(uint4 x) { return __hiloint2double((int)x.w, (int)x.z); }
+
+/* _simsimd_cos_normalize_f64_skylake (spatial.h:1544-1585) on the f64 sums themselves, restated in IEEE like the f32
+ * cosine (rsqrt14_pd + one Newton step differs by <= 1 ULP(f32) after the cast) */
+__device__ __forceinline__ float cos_normalize_wide_f64(double ab, double a2, double b2) {
+    if (a2 == 0 && b2 == 0) return 0.f;
+    if (ab == 0) return 1.f;
+    double ra = __drcp_rn(__dsqrt_rn(a2));
+    double rb = __drcp_rn(__dsqrt_rn(b2));
+    double r = __dsub_rn(1.0, __dmul_rn(__dmul_rn(ab, ra), rb));
+    return r > 0 ? __double2float_rn(r) : 0.f;
+}
+
+struct l2sq_f64_t {
+    static constexpr int LPV = 4;
+    static constexpr bool NORMS = false;
+    template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
+    template <class Q> static __device__ __forceinline__ float finalize_sw(float raw, Q, float) { return raw; }
+    struct acc_t { double v[2]; };
+    struct qconst_t {};
+    static __device__ __forceinline__ void init(acc_t& a) { a.v[0] = a.v[1] = 0.0; }
+    static __device__ __forceinline__ void step(acc_t& a, uint4 b, uint4 q) {
+        double const x0 = __dsub_rn(lo_f64(q), lo_f64(b)), x1 = __dsub_rn(hi_f64(q), hi_f64(b));
+        a.v[0] = __fma_rn(x0, x0, a.v[0]);
+        a.v[1] = __fma_rn(x1, x1, a.v[1]);
+    }
+    static __device__ __forceinline__ float finish(acc_t const& a, qconst_t) { return __double2float_rn(reduce8_lanes_f64(a.v[0], a.v[1])); }
+    static __device__ __forceinline__ qconst_t prepare(uint4 const*, uint32_t, int) { return {}; }
+};
+
+struct ip_f64_t {
+    static constexpr int LPV = 4;
+    static constexpr bool NORMS = false;
+    template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
+    template <class Q> static __device__ __forceinline__ float finalize_sw(float raw, Q, float) { return raw; }
+    struct acc_t { double v[2]; };
+    struct qconst_t {};
+    static __device__ __forceinline__ void init(acc_t& a) { a.v[0] = a.v[1] = 0.0; }
+    static __device__ __forceinline__ void step(acc_t& a, uint4 b, uint4 q) {
+        a.v[0] = __fma_rn(lo_f64(q), lo_f64(b), a.v[0]);
+        a.v[1] = __fma_rn(hi_f64(q), hi_f64(b), a.v[1]);
+    }
+    /* index_plugins.hpp:1914-1916: the f64 dot is cast to f32 before `1 - x` */
+    static __device__ __forceinline__ float finish(acc_t const& a, qconst_t) {
+        return __fsub_rn(1.0f, __double2float_rn(reduce8_lanes_f64(a.v[0], a.v[1])));
+    }
+    static __device__ __forceinline__ qconst_t prepare(uint4 const*, uint32_t, int) { return {}; }
+};
+
+struct cos_f64_t {
+    static constexpr int LPV = 4;
+    static constexpr bool NORMS = false;
+    template <class Q> static __device__ __forceinline__ float finalize(float raw, Q, float) { return raw; }
+    template <class Q> static __device__ __forceinline__ float finalize_sw(float raw, Q, float) { return raw; }
+    struct acc_t { double ab[2], b2[2]; };
+    struct qconst_t { double a2; };
+    static __device__ __forceinline__ void init(acc_t& a) { a.ab[0] = a.ab[1] = a.b2[0] = a.b2[1] = 0.0; }
+    static __device__ __forceinline__ void step(acc_t& a, uint4 b, uint4 q) {
+        double const b0 = lo_f64(b), b1 = hi_f64(b);
+        a.ab[0] = __fma_rn(lo_f64(q), b0, a.ab[0]);
+        a.ab[1] = __fma_rn(hi_f64(q), b1, a.ab[1]);
+        a.b2[0] = __fma_rn(b0, b0, a.b2[0]);
+        a.b2[1] = __fma_rn(b1, b1, a.b2[1]);
+    }
+    static __device__ __forceinline__ float finish(acc_t const& a, qconst_t qc) {
+        double const ab = reduce8_lanes_f64(a.ab[0], a.ab[1]), b2 = reduce8_lanes_f64(a.b2[0], a.b2[1]);
+        return cos_normalize_wide_f64(ab, qc.a2, b2);
+    }
+    /* metric(stored, query): exact_search_t's argument order (index_plugins.hpp:2112) */
+    static __device__ __forceinline__ float finish_sw(acc_t const& a, qconst_t qc) {
+        double const ab = reduce8_lanes_f64(a.ab[0], a.ab[1]), b2 = reduce8_lanes_f64(a.b2[0], a.b2[1]);
+        return cos_normalize_wide_f64(ab, b2, qc.a2);
+    }
+    /* dot(q, q) in the 8-accumulator order; every 4-lane group computes the same value */
+    static __device__ __forceinline__ qconst_t prepare(uint4 const* q4, uint32_t chunks16, int lane) {
+        double v0 = 0.0, v1 = 0.0;
+        for (uint32_t j = lane & 3; j < chunks16; j += 4) {
+            uint4 const q = q4[j];
+            double const q0 = lo_f64(q), q1 = hi_f64(q);
+            v0 = __fma_rn(q0, q0, v0);
+            v1 = __fma_rn(q1, q1, v1);
+        }
+        return {reduce8_lanes_f64(v0, v1)};
     }
 };
 

@@ -1253,6 +1253,8 @@ cudaError_t search_compute_shadow(device_index_t const& ix, float const* norms, 
 /*
  *  Which kernel serves which index:
  *    f32, vectors >= 256 B      STAGED, 4 lanes per vector, 8 resident warps per SM allowed by the register budget
+ *    f64                        the f32 layout (4 lanes per vector, two doubles per 16-byte chunk): STAGED from 256 B,
+ *                               DIRECT below; both compiled for 8 resident warps per SM
  *    f16 / bf16, >= 256 B       STAGED with the WORD metrics (4 lanes per vector split by accumulator) compiled for 16
  *                               resident warps per SM; one stage set up to 2 KB vectors (a quarter of the shared memory
  *                               per warp of one lane per vector in a single 32-slot set)
@@ -1292,6 +1294,11 @@ template <class M, bool STAGED, int MIN_CTAS> static cudaError_t occupancy_k(int
         if (ix.metric == METRIC_IP) return staged ? OP<ip_f32_t, true, 8> ARGS : OP<ip_f32_t, false, 16> ARGS;  \
         if (ix.metric == METRIC_COS) return staged ? OP<cos_f32_t, true, 8> ARGS : OP<cos_f32_t, false, 16> ARGS; \
         break;                                                                                                  \
+    case SCALAR_F64:                                                                                            \
+        if (ix.metric == METRIC_L2SQ) return staged ? OP<l2sq_f64_t, true, 8> ARGS : OP<l2sq_f64_t, false, 8> ARGS; \
+        if (ix.metric == METRIC_IP) return staged ? OP<ip_f64_t, true, 8> ARGS : OP<ip_f64_t, false, 8> ARGS;  \
+        if (ix.metric == METRIC_COS) return staged ? OP<cos_f64_t, true, 8> ARGS : OP<cos_f64_t, false, 8> ARGS; \
+        break;                                                                                                  \
     case SCALAR_F16:                                                                                            \
         if (ix.metric == METRIC_L2SQ) return staged ? OP<l2sq_halfw_t<f16_conv_t>, true, 16> ARGS : OP<l2sq_half_t<f16_conv_t>, false, 16> ARGS; \
         if (ix.metric == METRIC_IP) return staged ? OP<ip_halfw_t<f16_conv_t>, true, 16> ARGS : OP<ip_half_t<f16_conv_t>, false, 16> ARGS; \
@@ -1326,14 +1333,15 @@ int search_lanes_per_vector(device_index_t const&) { return 4; } /* every STAGED
  * units (each lane of a group reads its own chunk), 16 for word units (a group reads one chunk) */
 uint32_t search_stage_pad(device_index_t const& ix) { return is_half(ix) ? 16u : 64u; }
 int search_stage_slots(device_index_t const& ix) { return search_is_staged(ix) ? 8 : 0; }
-/* kernels compiled for 16 resident warps per SM: what the plan may count on */
+/* resident warps per SM the compiled kernel's registers allow (its MIN_CTAS): what the plan may count on */
 int search_max_warps_per_sm(device_index_t const& ix) {
+    if (ix.scalar == SCALAR_F64) return 8; /* both f64 kernels: 16 warps per SM would spill their f64 accumulators */
     if (!search_is_staged(ix)) return 24;
     return ix.scalar == SCALAR_F32 ? 8 : 16;
 }
 /* one stage set (no double buffering, more resident warps) for the short staged vectors of the 16-warp kernels */
 bool search_single_stage_set(device_index_t const& ix) {
-    return search_is_staged(ix) && ix.scalar != SCALAR_F32 && ix.vec_stride <= 2048;
+    return search_is_staged(ix) && ix.scalar != SCALAR_F32 && ix.scalar != SCALAR_F64 && ix.vec_stride <= 2048;
 }
 
 cudaError_t search_launch(device_index_t const& ix, search_args_t const& a, int blocks, size_t smem, cudaStream_t stream) {
@@ -1349,6 +1357,7 @@ cudaError_t search_occupancy(device_index_t const& ix, int* blocks_per_sm, size_
 bool search_supported(uint32_t metric, uint32_t scalar) {
     switch (scalar) {
     case SCALAR_F32:
+    case SCALAR_F64:
     case SCALAR_F16:
     case SCALAR_BF16:
     case SCALAR_I8: return metric == METRIC_L2SQ || metric == METRIC_IP || metric == METRIC_COS;
