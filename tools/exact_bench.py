@@ -22,21 +22,26 @@ def linkless_blob(base: np.ndarray, metric: str, scalar: str, d: int) -> np.ndar
     return np.frombuffer(b"".join(parts), dtype=np.uint8)
 
 
-n, d, nq, k = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3]), 10
-scalar = sys.argv[4] if len(sys.argv) > 4 else "f32"
-metric = sys.argv[5] if len(sys.argv) > 5 else "cos"
-base = datagen.to_scalar(datagen.latent(n, d, seed=1, rank=16), scalar)
-q = datagen.to_scalar(datagen.latent(nq, d, seed=2, rank=16), scalar)
-index = Index.restore(linkless_blob(base, metric, scalar, d))
-for rep in range(4):
+def main():
+    n, d, nq, k = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3]), 10
+    scalar = sys.argv[4] if len(sys.argv) > 4 else "f32"
+    metric = sys.argv[5] if len(sys.argv) > 5 else "cos"
+    base = datagen.to_scalar(datagen.latent(n, d, seed=1, rank=16), scalar)
+    q = datagen.to_scalar(datagen.latent(nq, d, seed=2, rank=16), scalar)
+    index = Index.restore(linkless_blob(base, metric, scalar, d))
+    for rep in range(4):
+        t = time.perf_counter()
+        m = index.search(q, k, exact=True)
+        dt = time.perf_counter() - t
+    pairs = n * nq
+    print(f"index.search(exact) n={n} d={d} nq={nq} {scalar}/{metric}: {dt*1e3:.1f} ms, {nq/dt:.0f} q/s, "
+          f"{pairs*d/dt/1e12:.2f} T multiply-adds/s")
     t = time.perf_counter()
-    m = index.search(q, k, exact=True)
+    f = exact_search(base, q, k, metric=metric, dtype=scalar)
     dt = time.perf_counter() - t
-pairs = n * nq
-print(f"index.search(exact) n={n} d={d} nq={nq} {scalar}/{metric}: {dt*1e3:.1f} ms, {nq/dt:.0f} q/s, "
-      f"{pairs*d/dt/1e12:.2f} T multiply-adds/s")
-t = time.perf_counter()
-f = exact_search(base, q, k, metric=metric, dtype=scalar)
-dt = time.perf_counter() - t
-print(f"exact_search (free, incl. H2D of {base.nbytes/1e9:.2f} GB): {dt*1e3:.1f} ms; distances equal: "
-      f"{np.array_equal(f.distances.view(np.uint32), m.distances.view(np.uint32))}")
+    print(f"exact_search (free, incl. H2D of {base.nbytes/1e9:.2f} GB): {dt*1e3:.1f} ms; distances equal: "
+          f"{np.array_equal(f.distances.view(np.uint32), m.distances.view(np.uint32))}")
+
+
+if __name__ == "__main__":
+    main()

@@ -24,7 +24,7 @@
 
 #include "device_index.h"
 #include "exact_args.h"
-#include "exact_i8.cuh"
+#include "exact_i8.h"
 #include "metrics.cuh"
 #include "warp_primitives.cuh"
 

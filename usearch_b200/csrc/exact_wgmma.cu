@@ -26,7 +26,7 @@
 
 #include "device_index.h"
 #include "exact_args.h"
-#include "exact_i8.cuh"
+#include "exact_i8.h"
 #include "warp_primitives.cuh"
 
 namespace usearch_b200 {
@@ -115,31 +115,16 @@ __device__ __noinline__ void list_insert(float* ld, uint32_t* ls, uint32_t& size
     size = new_size;
 }
 
-/* what one query row needs to filter and insert: its norm terms and the thresholds derived from the list's worst */
+/* what one query row needs to filter and insert: its norm terms and the filter's thresholds (exact_i8.h, where their
+ * soundness is derived) from the list's worst */
 template <uint32_t METRIC> struct row_t {
     uint32_t row;  /* 0..127 in the tile */
     bool live;
     int qa2;
     float qr;
-    int thr_i;     /* filter thresholds; while the list is not full everything passes */
-    float thr_f;
+    i8_filter_t<METRIC> filter;
 
-    __device__ __forceinline__ void thresholds(uint32_t size, uint32_t k, float worst) {
-        thr_i = INT32_MIN;
-        thr_f = -__int_as_float(0x7f800000);
-        if (size < k) return;
-        /* the list is full: a column can only enter with d <= worst. Slack: the int -> float conversions and the subtraction
-         * round by at most 1.5 ulp of the sum's magnitude (sums beyond 2^24 are not exact in f32); 4 ulps + 4 units allowed */
-        if constexpr (METRIC == METRIC_IP) { /* d = 1 - float(ab), non-increasing in ab */
-            float const t = __fsub_rd(1.0f, worst);
-            thr_i = __float2int_rd(t - fabsf(t) * 4.8e-7f) - 4;
-        } else if constexpr (METRIC == METRIC_L2SQ) /* d = float(a2 + b2 - 2ab) <= worst  <=>  2ab - b2 >= a2 - floor(worst) (- slack) */
-            thr_i = qa2 - (__float2int_ru(worst + fabsf(worst) * 4.8e-7f) + 4);
-        else { /* d = 1 - ab*qr*vr <= worst  <=>  ab*vr >= (1 - worst) / qr, lowered by a relative 1e-5 */
-            float const base = __fdiv_rn(__fsub_rn(1.0f, worst), qr);
-            thr_f = base - fabsf(base) * 1e-5f - 1e-30f;
-        }
-    }
+    __device__ __forceinline__ void thresholds(uint32_t size, uint32_t k, float worst) { filter.set_thresholds(size, k, worst, qa2, qr); }
 };
 
 /* accumulator layout of m64nNk32 (PTX ISA, wgmma "Matrix fragments for D"): warp w of the warpgroup, lane l holds, for column
@@ -155,10 +140,7 @@ __device__ __forceinline__ uint64_t filter_row(int const (&d)[128], row_t<METRIC
         for (int e = 0; e < 2; ++e) {
             uint32_t const col = 8u * j + col0 + e;
             int const v = d[4 * j + 2 * H + e];
-            bool maybe;
-            if constexpr (METRIC == METRIC_IP) maybe = v >= r.thr_i;
-            else if constexpr (METRIC == METRIC_L2SQ) maybe = 2 * v - b2[col] >= r.thr_i;
-            else maybe = !(__int2float_rn(v) * rn[col] < r.thr_f); /* a NaN (zero vector) passes */
+            bool maybe = r.filter.maybe(v, METRIC == METRIC_L2SQ ? b2[col] : 0, METRIC == METRIC_COS ? rn[col] : 0.f);
             maybe = maybe && ((mask[j >> 2] >> (col & 31u)) & 1u);
             pm |= maybe ? (1ull << (2 * j + e)) : 0ull;
         }
