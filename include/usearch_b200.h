@@ -235,6 +235,37 @@ size_t usearch_b200_shards_payload_bytes(size_t queries_count, size_t count);
 void usearch_b200_merge_topk(void const* payloads, int world, size_t queries_count, size_t count, usearch_key_t* keys,
                              usearch_distance_t* distances, uint32_t* counts, usearch_error_t* error);
 
+/* ---- additive: several indexes on one GPU searched as one (the reference's `Indexes`) ----------------------------- */
+
+/* A group of index handles, the reference's `Indexes` (python/lib.cpp:74-107, :321-402). The group borrows its members:
+ * they must outlive it, and it never frees them. The same handle may be merged more than once. A search gives what the
+ * reference's `Indexes.search` gives on one thread: every member searched in merge order (with its own expansion_search),
+ * each result folded into the query's row by search_result_t::merge_into (index.hpp:2650-2670). On data without NaN
+ * that is (distance ascending, later insertion first): a later member wins a tie. Members must share dimensions and
+ * device and must not be sharded handles. The call locks every distinct member for its duration, in ascending address
+ * order. */
+typedef void* usearch_b200_indexes_t;
+usearch_b200_indexes_t usearch_b200_indexes_init(usearch_error_t* error);
+void usearch_b200_indexes_free(usearch_b200_indexes_t indexes);
+void usearch_b200_indexes_merge(usearch_b200_indexes_t indexes, usearch_index_t index, usearch_error_t* error);
+/* the members' sizes summed (a handle merged twice counts twice, as in the reference) */
+size_t usearch_b200_indexes_size(usearch_b200_indexes_t indexes, usearch_error_t* error);
+/* Host buffers: `keys` / `distances` dense [queries_count x count], rows padded past counts[i] with key 0 and a signalling
+ * NaN. `computed_distances` / `visited_members` (may be NULL) receive per query the sums over members. A group without
+ * members answers with empty rows and no error. Returns the number of matches over all queries. */
+size_t usearch_b200_indexes_search_many(usearch_b200_indexes_t indexes, void const* queries, size_t queries_count,
+                                        size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count, bool exact,
+                                        usearch_key_t* keys, usearch_distance_t* distances, size_t* counts,
+                                        uint64_t* computed_distances, uint64_t* visited_members, usearch_error_t* error);
+/* Milliseconds of the last search, from CUDA events on the group's stream: member searches (queries upload included) |
+ * the merge kernel. */
+void usearch_b200_indexes_last_ms(usearch_b200_indexes_t indexes, float* out2);
+/* The merge kernel on host rows: `keys` / `distances` [shards x queries_count x count] and `counts` [shards x
+ * queries_count] (each clamped to count), folded shard by shard as usearch_b200_indexes_search_many folds them. */
+void usearch_b200_merge_into(usearch_key_t const* keys, usearch_distance_t const* distances, uint32_t const* counts, size_t shards,
+                             size_t queries_count, size_t count, usearch_key_t* merged_keys, usearch_distance_t* merged_distances,
+                             uint32_t* merged_counts, usearch_error_t* error);
+
 /* ---- additive, device-resident variants ---------------------------------------------------- */
 
 /* All pointers are DEVICE pointers on the index's GPU; `queries` must already be in the index's

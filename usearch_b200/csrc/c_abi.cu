@@ -597,6 +597,57 @@ void usearch_b200_merge_topk(void const* payloads, int world, size_t queries_cou
     set_error(error, shards_merge_host(payloads, world, queries_count, count, keys, distances, counts));
 }
 
+/* ---- several indexes on one GPU searched as one (python/lib.cpp:74-107, :321-402 `Indexes`) ----------------------- */
+
+usearch_b200_indexes_t usearch_b200_indexes_init(usearch_error_t* error) {
+    index_group_t* group = nullptr;
+    set_error(error, guarded([&]() -> char const* { group = index_group_create(); return nullptr; }));
+    return group;
+}
+
+void usearch_b200_indexes_free(usearch_b200_indexes_t indexes) { index_group_free(static_cast<index_group_t*>(indexes)); }
+
+void usearch_b200_indexes_merge(usearch_b200_indexes_t indexes, usearch_index_t index, usearch_error_t* error) {
+    if (!index) return set_error(error, "No index to merge");
+    set_error(error, guarded([&]() -> char const* {
+        index_group_merge(*static_cast<index_group_t*>(indexes), as_index(index));
+        return nullptr;
+    }));
+}
+
+size_t usearch_b200_indexes_size(usearch_b200_indexes_t indexes, usearch_error_t*) {
+    return index_group_size(*static_cast<index_group_t*>(indexes));
+}
+
+size_t usearch_b200_indexes_search_many(usearch_b200_indexes_t indexes, void const* queries, size_t queries_count,
+                                        size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count, bool exact,
+                                        usearch_key_t* keys, usearch_distance_t* distances, size_t* counts,
+                                        uint64_t* computed_distances, uint64_t* visited_members, usearch_error_t* error) {
+    uint32_t qs = scalar_to_char(query_kind);
+    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
+    size_t total = 0;
+    if (char const* e = guarded([&] {
+            return index_group_search(*static_cast<index_group_t*>(indexes), queries, queries_count, queries_stride, qs, count, exact,
+                                      keys, distances, counts, computed_distances, visited_members, &total);
+        })) {
+        set_error(error, e);
+        return 0;
+    }
+    return total;
+}
+
+void usearch_b200_indexes_last_ms(usearch_b200_indexes_t indexes, float* out2) {
+    std::memcpy(out2, index_group_last_ms(*static_cast<index_group_t*>(indexes)), 2 * sizeof(float));
+}
+
+void usearch_b200_merge_into(usearch_key_t const* keys, usearch_distance_t const* distances, uint32_t const* counts, size_t shards,
+                             size_t queries_count, size_t count, usearch_key_t* merged_keys, usearch_distance_t* merged_distances,
+                             uint32_t* merged_counts, usearch_error_t* error) {
+    set_error(error, guarded([&] {
+        return indexes_merge_host(keys, distances, counts, shards, queries_count, count, merged_keys, merged_distances, merged_counts);
+    }));
+}
+
 void usearch_clear(usearch_index_t index, usearch_error_t*) {
     frozen_index_t* ix = as_index(index);
     std::lock_guard<std::mutex> lock(ix->mutex);

@@ -286,6 +286,21 @@ char const* shards_unique_id(void* out128);
 size_t shards_payload_bytes(size_t nq, size_t k);
 char const* shards_merge_host(void const* payloads, int world, size_t nq, size_t k, uint64_t* keys, float* dists, uint32_t* counts);
 
+/* indexes.cu: several handles on one device searched as one, the reference's `Indexes` run on one thread. The group
+ * borrows its members (never frees them); one handle may be merged more than once. */
+struct index_group_t;
+index_group_t* index_group_create();
+void index_group_free(index_group_t* group);
+void index_group_merge(index_group_t& group, frozen_index_t* member);
+size_t index_group_size(index_group_t& group);
+float const* index_group_last_ms(index_group_t& group); /* searches | merge kernel of the last search, CUDA events */
+char const* index_group_search(index_group_t& group, void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                               bool exact, uint64_t* keys, float* dists, size_t* counts, uint64_t* computed, uint64_t* visited,
+                               size_t* total);
+/* merge_into of host rows: keys / dists [shards][nq][k], counts [shards][nq] -> [nq][k] and counts [nq] */
+char const* indexes_merge_host(uint64_t const* keys, float const* dists, uint32_t const* counts, size_t shards, size_t nq, size_t k,
+                               uint64_t* out_keys, float* out_dists, uint32_t* out_counts);
+
 /* builder.cu: scalar casts and single-pair distances on the device */
 char const* cast_rows_device(uint8_t const* src, size_t src_stride, uint32_t from, uint8_t* dst, size_t dst_stride, uint32_t to,
                              size_t dims, size_t rows, cudaStream_t stream);

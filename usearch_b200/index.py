@@ -56,7 +56,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_search_many_enqueue", "usearch_b200_search_many_finish", "usearch_b200_tune",
     "usearch_b200_launch_plan", "usearch_b200_remove_many", "usearch_b200_count_many", "usearch_b200_change_reuse_removed",
     "usearch_b200_reuse_removed", "usearch_b200_join", "usearch_b200_pairwise_distances",
-    "usearch_b200_last_join_ms",
+    "usearch_b200_last_join_ms", "usearch_b200_indexes_init", "usearch_b200_indexes_free", "usearch_b200_indexes_merge",
+    "usearch_b200_indexes_size", "usearch_b200_indexes_search_many", "usearch_b200_indexes_last_ms", "usearch_b200_merge_into",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -173,6 +174,18 @@ def load_library() -> C.CDLL:
     lib.usearch_b200_shards_payload_bytes.restype = C.c_size_t
     lib.usearch_b200_shards_payload_bytes.argtypes = [C.c_size_t, C.c_size_t]
     lib.usearch_b200_merge_topk.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_indexes_init.restype = C.c_void_p
+    lib.usearch_b200_indexes_init.argtypes = [err]
+    lib.usearch_b200_indexes_free.argtypes = [C.c_void_p]
+    lib.usearch_b200_indexes_merge.argtypes = [C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_indexes_size.restype = C.c_size_t
+    lib.usearch_b200_indexes_size.argtypes = [C.c_void_p, err]
+    lib.usearch_b200_indexes_search_many.restype = C.c_size_t
+    lib.usearch_b200_indexes_search_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t, C.c_bool,
+                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_indexes_last_ms.argtypes = [C.c_void_p, C.c_void_p]
+    lib.usearch_b200_merge_into.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, err]
     lib.usearch_distance.restype = C.c_float
     lib.usearch_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_size_t, C.c_int, err]
     _lib = lib
@@ -697,6 +710,117 @@ class Index:
                                                   counts_ptr, computed_ptr or None, visited_ptr or None,
                                                   stream or None, C.byref(err))
         _raise(err)
+
+
+class Indexes:
+    """Drop-in for ``usearch.index.Indexes`` (index.py:1473-1514): several indexes on one GPU searched as one.
+
+    ``search`` searches every member for every query, in merge order, and folds each member's result into the query's
+    row as the reference's ``search_result_t::merge_into`` does when ``Indexes.search`` runs on one thread: keys,
+    distance bits and counts equal that run's. On data without NaN the order is (distance ascending, later insertion
+    first), so a later member wins a tie. The members are borrowed: this object keeps the ``Index`` objects alive."""
+
+    def __init__(self, indexes=(), paths=(), view: bool = False, threads: int = 0):
+        del threads
+        self._lib = load_library()
+        err = C.c_char_p()
+        self._h = C.c_void_p(self._lib.usearch_b200_indexes_init(C.byref(err)))
+        _raise(err)
+        self._members = []
+        self._view = view
+        for index in indexes:
+            self.merge(index)
+        for path in paths:
+            self.merge_path(path)
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._lib.usearch_b200_indexes_free(self._h)
+            self._h = None
+
+    def merge(self, index: Index) -> None:
+        err = C.c_char_p()
+        self._lib.usearch_b200_indexes_merge(self._h, index._h, C.byref(err))
+        _raise(err)
+        self._members.append(index)
+
+    def merge_path(self, path) -> None:
+        """Restore the file at `path` onto the GPU and add it as the last member."""
+        self.merge(Index.restore(os.fspath(path), view=self._view))
+
+    def __len__(self) -> int:
+        return int(self._lib.usearch_b200_indexes_size(self._h, None))
+
+    @property
+    def last_ms(self) -> dict:
+        """Milliseconds of the last search from CUDA events: member searches (with the queries' upload), merge kernel."""
+        ms = np.zeros(2, dtype=np.float32)
+        self._lib.usearch_b200_indexes_last_ms(self._h, ms.ctypes.data_as(C.c_void_p))
+        return {"search": float(ms[0]), "merge": float(ms[1])}
+
+    def search(self, vectors, count: int = 10, *, threads: int = 0, exact: bool = False,
+               progress=None) -> Union[Matches, BatchMatches]:
+        """1-D input -> :class:`Matches`; 2-D input -> :class:`BatchMatches`. `visited_members` / `computed_distances`
+        are summed over members and queries; the per-query sums over members land in `last_computed` / `last_visited`.
+        `threads` and `progress` are accepted and ignored, as in `Index.search`."""
+        del threads, progress
+        vectors = np.asarray(vectors)
+        single = vectors.ndim == 1
+        if single:
+            vectors = vectors[None, :]
+        if vectors.ndim != 2:
+            raise ValueError("Expects a matrix or a vector")
+        if not vectors.flags.c_contiguous and vectors.strides[1] != vectors.itemsize:
+            vectors = np.ascontiguousarray(vectors)
+        if self._members:
+            first = self._members[0]
+            kind = first._kind_of(vectors)
+            expect_cols = (first.ndim * _BITS[kind] + 7) // 8 // vectors.itemsize if kind != "b1" else (first.ndim + 7) // 8
+            if vectors.shape[1] != expect_cols:
+                raise ValueError("The number of columns must match the dimensionality of the index")
+        else:
+            kind = "bf16" if vectors.dtype == np.uint16 else _NP_TO_SCALAR.get(vectors.dtype)
+            if kind is None:
+                raise TypeError(f"Unsupported query dtype {vectors.dtype}")
+        nq = vectors.shape[0]
+        keys = np.zeros((nq, count), dtype=np.uint64)
+        distances = np.zeros((nq, count), dtype=np.float32)
+        counts = np.zeros(nq, dtype=np.uint64)
+        computed = np.zeros(nq, dtype=np.uint64)
+        visited = np.zeros(nq, dtype=np.uint64)
+        err = C.c_char_p()
+        self._lib.usearch_b200_indexes_search_many(
+            self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count, bool(exact),
+            keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
+            computed.ctypes.data_as(C.c_void_p), visited.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        self.last_computed, self.last_visited = computed, visited
+        vm, cd = int(visited.sum()), int(computed.sum())
+        if single:
+            n = int(counts[0])
+            return Matches(keys[0, :n], distances[0, :n], vm, cd)
+        return BatchMatches(keys, distances, counts, vm, cd)
+
+
+def merge_into(keys: np.ndarray, distances: np.ndarray, counts: np.ndarray) -> BatchMatches:
+    """The merge kernel of :class:`Indexes` on host rows: `keys` [S, nq, count] u64, `distances` [S, nq, count] f32 and
+    `counts` [S, nq], folded member by member as the reference's `merge_into` folds them on one thread."""
+    lib = load_library()
+    keys = np.ascontiguousarray(keys, dtype=np.uint64)
+    distances = np.ascontiguousarray(distances, dtype=np.float32)
+    counts = np.ascontiguousarray(counts, dtype=np.uint32)
+    shards, nq, count = keys.shape
+    if distances.shape != keys.shape or counts.shape != (shards, nq):
+        raise ValueError("keys, distances and counts must be [S, nq, count], [S, nq, count] and [S, nq]")
+    out_keys = np.zeros((nq, count), dtype=np.uint64)
+    out_distances = np.zeros((nq, count), dtype=np.float32)
+    out_counts = np.zeros(nq, dtype=np.uint32)
+    err = C.c_char_p()
+    lib.usearch_b200_merge_into(keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p),
+                                counts.ctypes.data_as(C.c_void_p), shards, nq, count, out_keys.ctypes.data_as(C.c_void_p),
+                                out_distances.ctypes.data_as(C.c_void_p), out_counts.ctypes.data_as(C.c_void_p), C.byref(err))
+    _raise(err)
+    return BatchMatches(out_keys, out_distances, out_counts.astype(np.uint64))
 
 
 def exact_search(dataset: np.ndarray, queries: np.ndarray, count: int = 10, *, metric: str = "cos",
