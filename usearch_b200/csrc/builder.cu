@@ -674,19 +674,16 @@ char const* iota_u64_device(uint64_t* d_out, size_t n, cudaStream_t s) {
 
 namespace {
 
-template <typename T> char const* regrow(void*& slot, T const*& view, size_t old_count, size_t new_count, int fill_byte, cudaStream_t s) {
-    T* fresh = nullptr;
-    if (cudaMalloc(&fresh, std::max<size_t>(new_count, 1) * sizeof(T)) != cudaSuccess) {
-        cudaGetLastError();
-        return "Out of GPU memory!";
-    }
-    if (old_count) CU(cudaMemcpyAsync(fresh, view, old_count * sizeof(T), cudaMemcpyDeviceToDevice, s));
+template <typename T>
+char const* regrow(device_buffer_t<T>& array, T const*& view, size_t old_count, size_t new_count, int fill_byte, cudaStream_t s) {
+    device_buffer_t<T> fresh;
+    if (char const* e = fresh.reserve(std::max<size_t>(new_count, 1))) return e;
+    if (old_count) CU(cudaMemcpyAsync(fresh.ptr, view, old_count * sizeof(T), cudaMemcpyDeviceToDevice, s));
     if (new_count > old_count && fill_byte >= 0)
-        CU(cudaMemsetAsync(fresh + old_count, fill_byte, (new_count - old_count) * sizeof(T), s));
+        CU(cudaMemsetAsync(fresh.ptr + old_count, fill_byte, (new_count - old_count) * sizeof(T), s));
     CU(cudaStreamSynchronize(s));
-    if (slot) cudaFree(slot);
-    slot = fresh;
-    view = fresh;
+    array = std::move(fresh);
+    view = array.ptr;
     return nullptr;
 }
 
@@ -720,23 +717,21 @@ char const* frozen_index_t::reserve_slots(size_t slots) {
     size_t const rows_old = upper_capacity;
     /* expected upper rows: n / (M - 1); keep a quarter more, the rest grows on demand */
     size_t const rows_new = std::max<size_t>(rows_old, slots / std::max<size_t>(connectivity - 1, 1) * 5 / 4 + 1024);
-    uint8_t const* vec8 = d.vectors;
-    if (char const* e = regrow<uint8_t>(dev_allocs[0], vec8, old_cap * d.vec_stride, slots * d.vec_stride, -1, stream)) return e;
-    d.vectors = vec8;
-    if (char const* e = regrow<uint64_t>(dev_allocs[1], d.keys, old_cap, slots, -1, stream)) return e;
-    if (char const* e = regrow<uint32_t>(dev_allocs[2], d.nbr0, old_cap * d.m0_stride, slots * d.m0_stride, 0xFF, stream)) return e;
-    if (char const* e = regrow<uint32_t>(dev_allocs[3], d.upper_base, old_cap, slots, 0xFF, stream)) return e;
+    if (char const* e = regrow(hbm.vectors, d.vectors, old_cap * d.vec_stride, slots * d.vec_stride, -1, stream)) return e;
+    if (char const* e = regrow(hbm.keys, d.keys, old_cap, slots, -1, stream)) return e;
+    if (char const* e = regrow(hbm.nbr0, d.nbr0, old_cap * d.m0_stride, slots * d.m0_stride, 0xFF, stream)) return e;
+    if (char const* e = regrow(hbm.upper_base, d.upper_base, old_cap, slots, 0xFF, stream)) return e;
     if (rows_new > rows_old) {
-        if (char const* e = regrow<uint32_t>(dev_allocs[4], d.upper, rows_old * d.m_stride, rows_new * d.m_stride, 0xFF, stream)) return e;
+        if (char const* e = regrow(hbm.upper, d.upper, rows_old * d.m_stride, rows_new * d.m_stride, 0xFF, stream)) return e;
         upper_capacity = rows_new;
     }
     if (d.deleted_bits)
-        if (char const* e = regrow<uint32_t>(dev_allocs[5], d.deleted_bits, (old_cap + 31) / 32, (slots + 31) / 32, 0, stream)) return e;
+        if (char const* e = regrow(hbm.deleted_bits, d.deleted_bits, (old_cap + 31) / 32, (slots + 31) / 32, 0, stream)) return e;
     if (search_needs_norms(metric, scalar))
-        if (char const* e = regrow<float>(dev_allocs[6], d.norms, old_cap, slots, -1, stream)) return e;
+        if (char const* e = regrow(hbm.norms, d.norms, old_cap, slots, -1, stream)) return e;
     if (d.code_stride) { /* the int8 shadow of cos / ip f32 (prefilter_bound.h) */
-        if (char const* e = regrow<int8_t>(dev_allocs[8], d.codes, old_cap * d.code_stride, slots * d.code_stride, -1, stream)) return e;
-        if (char const* e = regrow<pf_record_t>(dev_allocs[9], d.shadow, old_cap, slots, -1, stream)) return e;
+        if (char const* e = regrow(hbm.codes, d.codes, old_cap * d.code_stride, slots * d.code_stride, -1, stream)) return e;
+        if (char const* e = regrow(hbm.shadow, d.shadow, old_cap, slots, -1, stream)) return e;
     }
     capacity = slots;
     hbm_bytes = capacity * (d.vec_stride + 8 + (size_t)d.m0_stride * 4 + 4 + (d.norms ? 4 : 0) +
@@ -749,7 +744,7 @@ char const* frozen_index_t::reserve_slots(size_t slots) {
 char const* frozen_index_t::reserve_upper_rows(size_t rows) {
     if (rows <= upper_capacity) return nullptr;
     size_t const rows_new = std::max(rows, upper_capacity * 2 + 1024);
-    if (char const* e = regrow<uint32_t>(dev_allocs[4], d.upper, upper_capacity * d.m_stride, rows_new * d.m_stride, 0xFF, stream)) return e;
+    if (char const* e = regrow(hbm.upper, d.upper, upper_capacity * d.m_stride, rows_new * d.m_stride, 0xFF, stream)) return e;
     upper_capacity = rows_new;
     return nullptr;
 }
@@ -800,12 +795,10 @@ char const* frozen_index_t::write_rows(void const* vectors, size_t rows, size_t 
 char const* frozen_index_t::set_slot_keys(uint32_t const* slots, size_t count, uint64_t const* keys) {
     if (!count) return nullptr;
     if (!d.deleted_bits) {
-        uint32_t* bits = nullptr;
         size_t const words = (capacity + 31) / 32;
-        CU(cudaMalloc(&bits, words * 4));
-        CU(cudaMemsetAsync(bits, 0, words * 4, stream));
-        dev_allocs[5] = bits;
-        d.deleted_bits = bits;
+        if (char const* e = hbm.deleted_bits.reserve(words)) return e;
+        CU(cudaMemsetAsync(hbm.deleted_bits.ptr, 0, words * 4, stream));
+        d.deleted_bits = hbm.deleted_bits.ptr;
         hbm_bytes += words * 4;
     }
     if (char const* e = edit_slots.reserve(count)) return e;
@@ -1088,7 +1081,7 @@ char const* frozen_index_t::link_batch(uint32_t const* slots, size_t count) {
     size_t const smem = off;
     if (smem > 200 * 1024) return "Dimensionality too large for the on-chip state of the builder";
     int const per_sm = (int)std::max<size_t>(1, std::min<size_t>(2048 / LINK_THREADS, (228 * 1024) / (smem + 1024)));
-    int const grid = per_sm * sm_count;
+    int const grid = per_sm * stream.sm_count;
     CU(cudaMemsetAsync(b.counters.ptr, 0, 16, s));
     la.work_counter = b.counters.ptr + 0;
     CU(launch_forward(d, la, (int)std::min<size_t>((size_t)grid, ntasks), smem, s));
@@ -1161,7 +1154,7 @@ char const* frozen_index_t::isolate(size_t* pruned) {
     if (char const* e = pruned_counter.reserve(1)) return e;
     CU(cudaMemsetAsync(pruned_counter.ptr, 0, 8, stream));
     size_t const rows = (size_t)d.n + upper_rows;
-    unsigned const blocks = (unsigned)std::min<size_t>((rows + 7) / 8, (size_t)sm_count * 8);
+    unsigned const blocks = (unsigned)std::min<size_t>((rows + 7) / 8, (size_t)stream.sm_count * 8);
     isolate_kernel<<<blocks, 256, 0, stream>>>(d, (uint32_t)upper_rows, pruned_counter.ptr);
     CU(cudaGetLastError());
     unsigned long long total = 0;

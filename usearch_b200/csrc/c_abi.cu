@@ -154,7 +154,7 @@ usearch_index_t usearch_init(usearch_init_options_t* options, usearch_error_t* e
         set_error(error, "Out of memory!");
         return nullptr;
     }
-    index->device = default_device();
+    index->stream.device = default_device();
     if (!options) return index; /* c/lib.cpp:142-147: empty index awaiting `load` */
     if (options->metric) {
         set_error(error, "Custom host metrics cannot run on the device");
@@ -694,7 +694,7 @@ int usearch_b200_launch_plan(usearch_index_t index, size_t count, uint64_t* out1
     return 0;
 }
 
-int usearch_b200_device(usearch_index_t index) { return as_index(index)->device; }
+int usearch_b200_device(usearch_index_t index) { return as_index(index)->stream.device; }
 uint64_t usearch_b200_kernel_launches(usearch_index_t index) { return as_index(index)->kernel_launches; }
 float usearch_b200_last_kernel_ms(usearch_index_t index) { return as_index(index)->last_kernel_ms; }
 size_t usearch_b200_bytes_per_vector(usearch_index_t index) { return as_index(index)->d.bytes_per_vector; }

@@ -3,7 +3,7 @@
  *  text from the calling function.
  */
 #pragma once
-#include <cuda_runtime.h>
+#include <cuda_runtime_api.h>
 
 #include <cstdio>
 

@@ -50,31 +50,8 @@ size_t bits_per_scalar(uint32_t s) { /* index_plugins.hpp:237-257 */
     }
 }
 
-frozen_index_t::~frozen_index_t() {
-    for (pending_search_t& p : pending) pending_free.push_back(p.status);
-    for (device_buffer_t<uint32_t>* b : pending_free) { b->release(); delete b; }
-    leave_shards();
-    release_device();
-    if (stream) cudaStreamDestroy(stream);
-    if (ev_begin) cudaEventDestroy(ev_begin);
-    if (ev_end) cudaEventDestroy(ev_end);
-    phase_cycles.release();
-    build.release();
-    cast_stage.release();
-    exact_scratch.release();
-    visit_log.release();
-    visited.release(); work_counter.release(); status.release(); counts.release(); computed.release();
-    cycles.release(); retry_list.release(); heap_spill.release(); queries.release(); out_keys.release();
-    allowed_keys.release(); allow_bits.release();
-    out_dists.release(); h_queries.release(); h_keys.release(); h_dists.release(); h_counts.release();
-    h_computed.release(); h_cycles.release(); h_status.release();
-}
-
 void frozen_index_t::release_device() {
-    for (void*& p : dev_allocs) {
-        if (p) cudaFree(p);
-        p = nullptr;
-    }
+    hbm = hbm_arrays_t{};
     d = device_index_t{};
     hbm_bytes = 0;
     loaded = false;
@@ -91,17 +68,10 @@ void frozen_index_t::release_device() {
 }
 
 char const* frozen_index_t::ensure_context() {
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-        cudaGetLastError();
-        return "No CUDA device: the GPU search backend has no CPU fallback";
-    }
-    CU(cudaSetDevice(device));
-    if (!stream) {
-        CU(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-        CU(cudaEventCreate(&ev_begin));
-        CU(cudaEventCreate(&ev_end));
-        CU(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device));
+    if (char const* e = stream.open()) return e;
+    if (!ev_end) {
+        CU(ev_begin.create());
+        CU(ev_end.create());
     }
     return nullptr;
 }
@@ -226,25 +196,22 @@ char const* frozen_index_t::load_blob(uint8_t const* blob, size_t length) {
     }
 
     /* device allocations */
-    uint8_t* d_vectors = nullptr;
-    uint64_t* d_keys = nullptr;
-    uint32_t *d_nbr0 = nullptr, *d_upper_base = nullptr, *d_upper = nullptr, *d_deleted = nullptr;
     size_t const bytes_vectors = (size_t)n * ix.vec_stride, bytes_keys = (size_t)n * 8,
                  bytes_nbr0 = (size_t)n * ix.m0_stride * 4, bytes_ub = (size_t)n * 4,
                  bytes_upper = std::max<size_t>(upper_rows, 1) * ix.m_stride * 4, bytes_deleted = ((size_t)n + 31) / 32 * 4;
-    CU(cudaMalloc(&d_vectors, bytes_vectors)); dev_allocs[0] = d_vectors;
-    CU(cudaMalloc(&d_keys, bytes_keys)); dev_allocs[1] = d_keys;
-    CU(cudaMalloc(&d_nbr0, bytes_nbr0)); dev_allocs[2] = d_nbr0;
-    CU(cudaMalloc(&d_upper_base, bytes_ub)); dev_allocs[3] = d_upper_base;
-    CU(cudaMalloc(&d_upper, bytes_upper)); dev_allocs[4] = d_upper;
+    if (char const* e = hbm.vectors.reserve(bytes_vectors)) return e;
+    if (char const* e = hbm.keys.reserve(n)) return e;
+    if (char const* e = hbm.nbr0.reserve((size_t)n * ix.m0_stride)) return e;
+    if (char const* e = hbm.upper_base.reserve(n)) return e;
+    if (char const* e = hbm.upper.reserve(std::max<size_t>(upper_rows, 1) * ix.m_stride)) return e;
     hbm_bytes = bytes_vectors + bytes_keys + bytes_nbr0 + bytes_ub + bytes_upper;
 
     /* vectors: slot-major matrix, rows padded to 16 bytes */
     if (ix.vec_stride == bpv) {
-        CU(cudaMemcpy(d_vectors, matrix, bytes_vectors, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(hbm.vectors.ptr, matrix, bytes_vectors, cudaMemcpyHostToDevice));
     } else {
-        CU(cudaMemset(d_vectors, 0, bytes_vectors));
-        CU(cudaMemcpy2D(d_vectors, ix.vec_stride, matrix, bpv, bpv, n, cudaMemcpyHostToDevice));
+        CU(cudaMemset(hbm.vectors.ptr, 0, bytes_vectors));
+        CU(cudaMemcpy2D(hbm.vectors.ptr, ix.vec_stride, matrix, bpv, bpv, n, cudaMemcpyHostToDevice));
     }
 
     /* pass 2: node tapes -> keys, nbr0 rows, upper rows; converted and uploaded in chunks */
@@ -297,42 +264,39 @@ char const* frozen_index_t::load_blob(uint8_t const* blob, size_t length) {
             }
             q = list;
         }
-        CU(cudaMemcpy(d_keys + begin, h_keys.data(), (stop - begin) * 8, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_nbr0 + begin * ix.m0_stride, h_nbr0.data(), (stop - begin) * ix.m0_stride * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(hbm.keys.ptr + begin, h_keys.data(), (stop - begin) * 8, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(hbm.nbr0.ptr + begin * ix.m0_stride, h_nbr0.data(), (stop - begin) * ix.m0_stride * 4, cudaMemcpyHostToDevice));
         if (chunk_upper_rows)
-            CU(cudaMemcpy(d_upper + first_upper_row * ix.m_stride, h_upper.data(), chunk_upper_rows * ix.m_stride * 4,
+            CU(cudaMemcpy(hbm.upper.ptr + first_upper_row * ix.m_stride, h_upper.data(), chunk_upper_rows * ix.m_stride * 4,
                           cudaMemcpyHostToDevice));
     }
-    CU(cudaMemcpy(d_upper_base, upper_base.data(), bytes_ub, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(hbm.upper_base.ptr, upper_base.data(), bytes_ub, cudaMemcpyHostToDevice));
     if (any_deleted) {
-        CU(cudaMalloc(&d_deleted, bytes_deleted)); dev_allocs[5] = d_deleted;
-        CU(cudaMemcpy(d_deleted, h_deleted.data(), bytes_deleted, cudaMemcpyHostToDevice));
+        if (char const* e = hbm.deleted_bits.reserve(bytes_deleted / 4)) return e;
+        CU(cudaMemcpy(hbm.deleted_bits.ptr, h_deleted.data(), bytes_deleted, cudaMemcpyHostToDevice));
         hbm_bytes += bytes_deleted;
     }
-    ix.vectors = d_vectors;
-    ix.keys = d_keys;
-    ix.nbr0 = d_nbr0;
-    ix.upper_base = d_upper_base;
-    ix.upper = d_upper;
-    ix.deleted_bits = d_deleted;
+    ix.vectors = hbm.vectors.ptr;
+    ix.keys = hbm.keys.ptr;
+    ix.nbr0 = hbm.nbr0.ptr;
+    ix.upper_base = hbm.upper_base.ptr;
+    ix.upper = hbm.upper.ptr;
+    ix.deleted_bits = hbm.deleted_bits.ptr;
     if (search_needs_norms(head_metric, head_scalar)) {
-        float* d_norms = nullptr;
-        CU(cudaMalloc(&d_norms, (size_t)n * 4)); dev_allocs[6] = d_norms;
+        if (char const* e = hbm.norms.reserve(n)) return e;
         hbm_bytes += (size_t)n * 4;
-        CU(search_compute_norms(ix, d_norms, stream));
+        CU(search_compute_norms(ix, hbm.norms.ptr, stream));
         CU(cudaStreamSynchronize(stream));
-        ix.norms = d_norms;
+        ix.norms = hbm.norms.ptr;
     }
     if (ix.code_stride) {
-        int8_t* d_codes = nullptr;
-        pf_record_t* d_shadow = nullptr;
-        CU(cudaMalloc(&d_codes, (size_t)n * ix.code_stride)); dev_allocs[8] = d_codes;
-        CU(cudaMalloc(&d_shadow, (size_t)n * sizeof(pf_record_t))); dev_allocs[9] = d_shadow;
+        if (char const* e = hbm.codes.reserve((size_t)n * ix.code_stride)) return e;
+        if (char const* e = hbm.shadow.reserve(n)) return e;
         hbm_bytes += (size_t)n * (ix.code_stride + sizeof(pf_record_t));
-        CU(search_compute_shadow(ix, ix.norms, d_codes, d_shadow, stream));
+        CU(search_compute_shadow(ix, ix.norms, hbm.codes.ptr, hbm.shadow.ptr, stream));
         CU(cudaStreamSynchronize(stream));
-        ix.codes = d_codes;
-        ix.shadow = d_shadow;
+        ix.codes = hbm.codes.ptr;
+        ix.shadow = hbm.shadow.ptr;
     }
     drop_host_state.armed = false;
     commit(ix, upper_rows);
@@ -353,7 +317,7 @@ size_t frozen_index_t::serialized_length() const {
  * index.hpp:3276-3317) by downloading the SoA arrays. */
 char const* frozen_index_t::save_blob(uint8_t* out, size_t length) const {
     if (length < serialized_length()) return "Failed to serialize into stream";
-    CU(cudaSetDevice(device));
+    CU(cudaSetDevice(stream.device));
     size_t const n = size, bpv = d.bytes_per_vector;
     uint8_t* p = out;
     uint32_t dims32[2] = {(uint32_t)n, (uint32_t)bpv};
@@ -518,8 +482,8 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
         return v && std::atoi(v) > 0 ? (uint64_t)std::atoi(v) : (uint64_t)1;
     }();
     uint64_t const bitmap_words = round_up((uint32_t)((visit_slots + 31) / 32), 4);
-    uint64_t const max_warps_guess = (uint64_t)sm_count * 32;
-    bool const bitmaps_fit = bitmap_words * 4 * std::min<uint64_t>(max_warps_guess, (uint64_t)sm_count * pl.warps_per_sm_target) <= BITMAP_SCRATCH_BUDGET;
+    uint64_t const max_warps_guess = (uint64_t)stream.sm_count * 32;
+    bool const bitmaps_fit = bitmap_words * 4 * std::min<uint64_t>(max_warps_guess, (uint64_t)stream.sm_count * pl.warps_per_sm_target) <= BITMAP_SCRATCH_BUDGET;
     if (forced == 2 || forced == 3 || (forced == 0 && bitmaps_fit)) {
         /* BITMAP visits: one bit per slot, exact, never overflows */
         pl.visited_bitmap_words = (uint32_t)bitmap_words;
@@ -544,7 +508,7 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     CU(search_occupancy(d, &per_sm, pl.smem_per_block));
     if (per_sm < 1) return "Kernel does not fit on an SM";
     per_sm = std::min<int>(per_sm, (int)pl.warps_per_sm_target);
-    pl.blocks = per_sm * sm_count;
+    pl.blocks = per_sm * stream.sm_count;
     return nullptr;
 }
 
@@ -612,12 +576,11 @@ char const* frozen_index_t::search_device(void const* d_queries, size_t nq, size
     if (char const* e = h_status.reserve(nq)) return e;
     uint32_t* status_ptr = nullptr;
     if (defer) { /* every batch in flight owns its status words until search_finish has looked at them */
-        if (pending_free.empty()) pending_free.emplace_back(new device_buffer_t<uint32_t>());
-        device_buffer_t<uint32_t>* buf = pending_free.back();
-        pending_free.pop_back();
-        if (char const* e = buf->reserve(nq)) { pending_free.push_back(buf); return e; }
-        pending.push_back(pending_search_t{buf, search_args_t{}, pl.maxed, s});
-        status_ptr = buf->ptr;
+        if (pending_status.size() == pending.size()) pending_status.emplace_back();
+        device_buffer_t<uint32_t>& buf = pending_status[pending.size()];
+        if (char const* e = buf.reserve(nq)) return e;
+        pending.push_back(pending_search_t{buf.ptr, search_args_t{}, pl.maxed, s});
+        status_ptr = buf.ptr;
     } else {
         if (char const* e = status.reserve(nq)) return e;
         status_ptr = status.ptr;
@@ -662,10 +625,9 @@ char const* frozen_index_t::search_finish() {
     for (pending_search_t& p : pending) {
         char const* e = cuda_error(cudaStreamSynchronize(p.stream));
         if (!e) e = h_status.reserve(p.args.nq);
-        if (!e) e = cuda_error(cudaMemcpy(h_status.ptr, p.status->ptr, (size_t)p.args.nq * 4, cudaMemcpyDeviceToHost));
+        if (!e) e = cuda_error(cudaMemcpy(h_status.ptr, p.status, (size_t)p.args.nq * 4, cudaMemcpyDeviceToHost));
         if (!e) e = retry_overflowed(p.args, p.maxed, p.stream);
         if (e && !first_error) first_error = e;
-        pending_free.push_back(p.status);
     }
     pending.clear();
     if (ev_begin && ev_end && !first_error) cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end);
@@ -977,7 +939,7 @@ char const* frozen_index_t::exact_host(void const* q, size_t nq, size_t stride, 
     if (char const* e = out_dists.reserve(nq * k)) return e;
     if (char const* e = counts_reserve_all(nq)) return e;
     if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
-    if (char const* e = exact_search_device(d, sm_count, queries.ptr, nq, vs, k, false, false, out_keys.ptr, out_dists.ptr, counts.ptr,
+    if (char const* e = exact_search_device(d, stream.sm_count, queries.ptr, nq, vs, k, false, false, out_keys.ptr, out_dists.ptr, counts.ptr,
                                             exact_scratch, stream))
         return e;
     kernel_launches += 2;
@@ -998,9 +960,8 @@ char const* exact_search_free(void const* dataset, size_t n, size_t dataset_stri
     if (!nq || !k) return nullptr;
     if (k > n) return "More neighbours requested than the dataset holds";
     if (n >= 0xFFFFFFFFull) return "Too many entries for 32-bit slots";
-    frozen_index_t tmp;
-    tmp.device = default_device();
-    if (char const* e = tmp.ensure_context()) return e;
+    cuda_stream_t s(default_device());
+    if (char const* e = s.open()) return e;
     size_t const bpv = (dimensions * bits_per_scalar(scalar) + 7) / 8, vs = (bpv + 15) / 16 * 16;
     device_index_t ix;
     ix.n = (uint32_t)n;
@@ -1014,16 +975,11 @@ char const* exact_search_free(void const* dataset, size_t n, size_t dataset_stri
     device_buffer_t<float> d_norms, d_dists;
     device_buffer_t<uint64_t> d_keys;
     device_buffer_t<uint32_t> d_counts;
-    struct release_all_t {
-        device_buffer_t<uint8_t>&a, &b, &c; device_buffer_t<float>&d, &e; device_buffer_t<uint64_t>& f; device_buffer_t<uint32_t>& g;
-        ~release_all_t() { a.release(); b.release(); c.release(); d.release(); e.release(); f.release(); g.release(); }
-    } release_all{d_vectors, d_queries, scratch, d_norms, d_dists, d_keys, d_counts};
     if (char const* e = d_vectors.reserve(n * vs)) return e;
     if (char const* e = d_queries.reserve(nq * vs)) return e;
     if (char const* e = d_keys.reserve(nq * k)) return e;
     if (char const* e = d_dists.reserve(nq * k)) return e;
     if (char const* e = d_counts.reserve(nq)) return e;
-    cudaStream_t s = tmp.stream;
     if (vs != bpv) {
         CU(cudaMemsetAsync(d_vectors.ptr, 0, n * vs, s));
         CU(cudaMemsetAsync(d_queries.ptr, 0, nq * vs, s));
@@ -1036,7 +992,7 @@ char const* exact_search_free(void const* dataset, size_t n, size_t dataset_stri
         CU(search_compute_norms(ix, d_norms.ptr, s));
         ix.norms = d_norms.ptr;
     }
-    if (char const* e = exact_search_device(ix, tmp.sm_count, d_queries.ptr, nq, vs, k, true, true, d_keys.ptr, d_dists.ptr, d_counts.ptr,
+    if (char const* e = exact_search_device(ix, s.sm_count, d_queries.ptr, nq, vs, k, true, true, d_keys.ptr, d_dists.ptr, d_counts.ptr,
                                             scratch, s))
         return e;
     CU(cudaMemcpy2DAsync(keys, keys_stride, d_keys.ptr, k * 8, k * 8, nq, cudaMemcpyDeviceToHost, s));
@@ -1047,9 +1003,8 @@ char const* exact_search_free(void const* dataset, size_t n, size_t dataset_stri
 
 /* usearch_distance: both vectors to the device, one warp, the metric struct of the search kernels */
 char const* pair_distance_host(void const* a, void const* b, uint32_t scalar, size_t dimensions, uint32_t metric, float* result) {
-    frozen_index_t tmp;
-    tmp.device = default_device();
-    if (char const* e = tmp.ensure_context()) return e;
+    cuda_stream_t s(default_device());
+    if (char const* e = s.open()) return e;
     size_t const bpv = (dimensions * bits_per_scalar(scalar) + 7) / 8, vs = (bpv + 15) / 16 * 16;
     if (vs > 48 * 1024) return "Vector too long for a single-pair distance";
     device_index_t ix;
@@ -1061,15 +1016,14 @@ char const* pair_distance_host(void const* a, void const* b, uint32_t scalar, si
     ix.scalar = scalar;
     device_buffer_t<uint8_t> pair;
     device_buffer_t<float> out;
-    struct release_t { device_buffer_t<uint8_t>& a; device_buffer_t<float>& b; ~release_t() { a.release(); b.release(); } } release{pair, out};
     if (char const* e = pair.reserve(2 * vs)) return e;
     if (char const* e = out.reserve(1)) return e;
-    CU(cudaMemsetAsync(pair.ptr, 0, 2 * vs, tmp.stream));
-    CU(cudaMemcpyAsync(pair.ptr, a, bpv, cudaMemcpyHostToDevice, tmp.stream));
-    CU(cudaMemcpyAsync(pair.ptr + vs, b, bpv, cudaMemcpyHostToDevice, tmp.stream));
-    if (char const* e = pair_distance_device(ix, pair.ptr, pair.ptr + vs, out.ptr, tmp.stream)) return e;
-    CU(cudaMemcpyAsync(result, out.ptr, 4, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaStreamSynchronize(tmp.stream));
+    CU(cudaMemsetAsync(pair.ptr, 0, 2 * vs, s));
+    CU(cudaMemcpyAsync(pair.ptr, a, bpv, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(pair.ptr + vs, b, bpv, cudaMemcpyHostToDevice, s));
+    if (char const* e = pair_distance_device(ix, pair.ptr, pair.ptr + vs, out.ptr, s)) return e;
+    CU(cudaMemcpyAsync(result, out.ptr, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
     return nullptr;
 }
 

@@ -15,6 +15,7 @@
 #include <string>
 #include <vector>
 
+#include "cuda_buffers.h"
 #include "device_index.h"
 #include "key_map.h"
 
@@ -64,50 +65,6 @@ struct launch_plan_t {
     size_t warps() const { return (size_t)blocks * (size_t)search_warps_per_block(); }
 };
 
-template <typename T> struct device_buffer_t {
-    T* ptr = nullptr;
-    size_t capacity = 0; /* elements */
-    char const* reserve(size_t n) {
-        if (n <= capacity) return nullptr;
-        if (ptr) cudaFree(ptr);
-        ptr = nullptr;
-        capacity = 0;
-        if (cudaMalloc(&ptr, n * sizeof(T)) != cudaSuccess) {
-            cudaGetLastError();
-            return "Out of GPU memory!";
-        }
-        capacity = n;
-        return nullptr;
-    }
-    void release() {
-        if (ptr) cudaFree(ptr);
-        ptr = nullptr;
-        capacity = 0;
-    }
-};
-
-template <typename T> struct pinned_buffer_t {
-    T* ptr = nullptr;
-    size_t capacity = 0;
-    char const* reserve(size_t n) {
-        if (n <= capacity) return nullptr;
-        if (ptr) cudaFreeHost(ptr);
-        ptr = nullptr;
-        capacity = 0;
-        if (cudaHostAlloc(&ptr, n * sizeof(T), cudaHostAllocDefault) != cudaSuccess) {
-            cudaGetLastError();
-            return "Out of pinned host memory!";
-        }
-        capacity = n;
-        return nullptr;
-    }
-    void release() {
-        if (ptr) cudaFreeHost(ptr);
-        ptr = nullptr;
-        capacity = 0;
-    }
-};
-
 /* device scratch of the batched builder (builder.cu) */
 struct build_scratch_t {
     device_buffer_t<uint32_t> task_slot, cand_slots, cand_counts, pair_idx, pair_idx_sorted, heads, counters;
@@ -115,12 +72,6 @@ struct build_scratch_t {
     device_buffer_t<float> cand_dists, pair_dists;
     device_buffer_t<uint64_t> pair_keys, pair_keys_sorted;
     size_t iota_count = 0;
-    void release() {
-        task_slot.release(); cand_slots.release(); cand_counts.release(); pair_idx.release(); pair_idx_sorted.release();
-        heads.release(); counters.release(); task_level.release(); sort_temp.release(); cand_dists.release();
-        pair_dists.release(); pair_keys.release(); pair_keys_sorted.release();
-        iota_count = 0;
-    }
 };
 
 struct shard_group_t; /* shards.cu */
@@ -149,11 +100,18 @@ struct frozen_index_t {
     void build_key_map() { if (!key_map.built) key_map.rebuild(host_keys, free_key, capacity); }
 
     /* device */
-    int device = 0;
-    device_index_t d;
+    cuda_stream_t stream; /* the handle's device (`stream.device`), its SM count and the handle's own stream */
+    device_index_t d;     /* views of the arrays in `hbm` */
     size_t hbm_bytes = 0;
     bool loaded = false;
-    void* dev_allocs[10] = {nullptr}; /* vectors keys nbr0 upper_base upper deleted norms - codes shadow */
+    struct hbm_arrays_t {
+        device_buffer_t<uint8_t> vectors;
+        device_buffer_t<uint64_t> keys;
+        device_buffer_t<uint32_t> nbr0, upper_base, upper, deleted_bits;
+        device_buffer_t<float> norms;
+        device_buffer_t<int8_t> codes;
+        device_buffer_t<pf_record_t> shadow;
+    } hbm;
 
     /* tuning knobs of the search launch: environment at construction (USEARCH_B200_STAGE_SETS, _WARPS_PER_SM,
      * _PREFILTER, _HEAP_HEAD), changeable per handle with usearch_b200_tune (bench sweeps, tests) */
@@ -171,8 +129,7 @@ struct frozen_index_t {
 
     /* per-handle execution context */
     std::mutex mutex;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
+    cuda_event_t ev_begin, ev_end;
     device_buffer_t<uint32_t> visited, visit_log, work_counter, status, counts, computed, cycles, retry_list;
     size_t visited_zeroed_words = 0; /* the first this-many words of `visited` are known to be zero (logged bitmaps) */
     device_buffer_t<cand_t> heap_spill;
@@ -191,9 +148,8 @@ struct frozen_index_t {
     bool profile_phases = false;
     uint64_t kernel_launches = 0;
     float last_kernel_ms = 0.f;
-    int sm_count = 0;
 
-    ~frozen_index_t();
+    ~frozen_index_t() { leave_shards(); } /* the NCCL communicator before the stream and buffers it uses */
     void release_device();
     char const* ensure_context();
     char const* counts_reserve_all(size_t nq);
@@ -246,9 +202,9 @@ struct frozen_index_t {
     char const* search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t* d_keys, float* d_dists,
                               uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles, cudaStream_t stream, bool defer = false);
     /* deferred launches (usearch_b200_search_many_enqueue): status words and arguments kept until search_finish */
-    struct pending_search_t { device_buffer_t<uint32_t>* status; search_args_t args; bool maxed; cudaStream_t stream; };
+    struct pending_search_t { uint32_t* status; search_args_t args; bool maxed; cudaStream_t stream; };
     std::vector<pending_search_t> pending;
-    std::vector<device_buffer_t<uint32_t>*> pending_free;
+    std::vector<device_buffer_t<uint32_t>> pending_status; /* pending[i] writes to pending_status[i]; the rest are free */
     char const* search_finish();
     char const* retry_overflowed(search_args_t const& a, bool maxed, cudaStream_t stream);
     /* usearch_search from many host threads: callers that arrive while a launch is in flight are gathered and served by

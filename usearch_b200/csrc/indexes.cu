@@ -138,9 +138,8 @@ struct query_rows_t {
 struct index_group_t {
     std::vector<frozen_index_t*> members; /* borrowed, in merge order; the same handle may appear more than once */
     std::mutex mutex;                     /* one search (or merge) of the group at a time */
-    int device = -1;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_begin = nullptr, ev_merge = nullptr, ev_end = nullptr;
+    cuda_stream_t stream;
+    cuda_event_t ev_begin, ev_merge, ev_end;
     float last_ms[2] = {0.f, 0.f}; /* searches | merge kernel, of the last search */
     device_buffer_t<uint8_t> raw_queries;
     std::vector<query_rows_t> casts;
@@ -150,31 +149,18 @@ struct index_group_t {
     device_buffer_t<uint8_t> merged; /* keys u64[nq*k] | computed u64[nq] | visited u64[nq] | distances f32[nq*k] | counts u32[nq] */
     pinned_buffer_t<uint8_t> h_merged;
 
-    ~index_group_t() { release(); }
-    void release() {
-        if (stream) {
-            cudaSetDevice(device);
-            cudaStreamDestroy(stream);
-            cudaEventDestroy(ev_begin);
-            cudaEventDestroy(ev_merge);
-            cudaEventDestroy(ev_end);
-        }
-        stream = nullptr;
+    char const* ensure_stream(int on_device) {
+        if (stream && stream.device == on_device) return nullptr;
+        /* the device scratch of the previous device cannot serve this one */
         raw_queries.release();
-        for (query_rows_t& c : casts) c.rows.release();
         casts.clear();
         keys.release(); dists.release(); counts.release(); computed.release(); visited.release(); merged.release();
         h_merged.release();
-    }
-    char const* ensure_stream(int on_device) {
-        if (stream && device == on_device) return nullptr;
-        release();
-        device = on_device;
-        CU(cudaSetDevice(device));
-        CU(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-        CU(cudaEventCreate(&ev_begin));
-        CU(cudaEventCreate(&ev_merge));
-        CU(cudaEventCreate(&ev_end));
+        stream = cuda_stream_t(on_device);
+        if (char const* e = stream.open()) return e;
+        CU(ev_begin.create());
+        CU(ev_merge.create());
+        CU(ev_end.create());
         return nullptr;
     }
     /* the raw queries in `scalar` with rows `stride` bytes apart (zero-padded), cast on the device once per kind */
@@ -244,7 +230,7 @@ char const* index_group_t::search(void const* q, size_t nq, size_t stride, uint3
     size_t const dims = members[0]->dimensions;
     for (frozen_index_t* m : members) {
         if (m->dimensions != dims) return "Can't search indexes of different dimensions together";
-        if (m->device != members[0]->device) return "Can't search indexes that live on different devices together";
+        if (m->stream.device != members[0]->stream.device) return "Can't search indexes that live on different devices together";
         if (m->shards) return "Can't search a sharded handle in Indexes: it holds one shard of its index";
     }
     /* every distinct handle for the whole call, in ascending address order, as join does: no two calls can deadlock */
@@ -255,7 +241,7 @@ char const* index_group_t::search(void const* q, size_t nq, size_t stride, uint3
     locks.reserve(distinct.size());
     for (frozen_index_t* m : distinct) locks.emplace_back(m->mutex);
 
-    if (char const* e = ensure_stream(members[0]->device)) return e;
+    if (char const* e = ensure_stream(members[0]->stream.device)) return e;
     cudaStream_t const s = stream;
     size_t const src_bytes = (dims * bits_per_scalar(query_scalar) + 7) / 8;
     if (!src_bytes) return "Unknown scalar kind!";
@@ -292,7 +278,7 @@ char const* index_group_t::search(void const* q, size_t nq, size_t stride, uint3
         uint8_t const* rows = nullptr;
         if (char const* e = rows_for(m.scalar, m.d.vec_stride, query_scalar, src_bytes, nq, dims, rows)) return e;
         if (exact) {
-            if (char const* e = exact_search_device(m.d, m.sm_count, rows, nq, m.d.vec_stride, k, false, false, sk, sd, sc,
+            if (char const* e = exact_search_device(m.d, m.stream.sm_count, rows, nq, m.d.vec_stride, k, false, false, sk, sd, sc,
                                                     m.exact_scratch, s))
                 return e;
             m.kernel_launches += 2;
@@ -348,17 +334,12 @@ char const* index_group_t::search(void const* q, size_t nq, size_t stride, uint3
 char const* indexes_merge_host(uint64_t const* keys, float const* dists, uint32_t const* counts, size_t shards, size_t nq, size_t k,
                                uint64_t* out_keys, float* out_dists, uint32_t* out_counts) {
     if (!nq || !k) return nullptr;
-    frozen_index_t tmp;
-    tmp.device = default_device();
-    if (char const* e = tmp.ensure_context()) return e;
+    cuda_stream_t s(default_device());
+    if (char const* e = s.open()) return e;
     size_t const rows = std::max<size_t>(shards, 1) * nq;
     device_buffer_t<uint64_t> dk, ok;
     device_buffer_t<float> dd, od;
     device_buffer_t<uint32_t> dc, oc;
-    struct release_t {
-        device_buffer_t<uint64_t>&a, &b; device_buffer_t<float>&c, &d; device_buffer_t<uint32_t>&e, &f;
-        ~release_t() { a.release(); b.release(); c.release(); d.release(); e.release(); f.release(); }
-    } release{dk, ok, dd, od, dc, oc};
     if (char const* e = dk.reserve(rows * k)) return e;
     if (char const* e = dd.reserve(rows * k)) return e;
     if (char const* e = dc.reserve(rows)) return e;
@@ -366,17 +347,17 @@ char const* indexes_merge_host(uint64_t const* keys, float const* dists, uint32_
     if (char const* e = od.reserve(nq * k)) return e;
     if (char const* e = oc.reserve(nq)) return e;
     if (shards) {
-        CU(cudaMemcpyAsync(dk.ptr, keys, shards * nq * k * 8, cudaMemcpyHostToDevice, tmp.stream));
-        CU(cudaMemcpyAsync(dd.ptr, dists, shards * nq * k * 4, cudaMemcpyHostToDevice, tmp.stream));
-        CU(cudaMemcpyAsync(dc.ptr, counts, shards * nq * 4, cudaMemcpyHostToDevice, tmp.stream));
+        CU(cudaMemcpyAsync(dk.ptr, keys, shards * nq * k * 8, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(dd.ptr, dists, shards * nq * k * 4, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(dc.ptr, counts, shards * nq * 4, cudaMemcpyHostToDevice, s));
     }
     if (char const* e = merge_into_launch(dk.ptr, dd.ptr, dc.ptr, nullptr, nullptr, shards, nq, k, ok.ptr, od.ptr, oc.ptr, nullptr,
-                                          nullptr, tmp.stream))
+                                          nullptr, s))
         return e;
-    CU(cudaMemcpyAsync(out_keys, ok.ptr, nq * k * 8, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaMemcpyAsync(out_dists, od.ptr, nq * k * 4, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaMemcpyAsync(out_counts, oc.ptr, nq * 4, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaStreamSynchronize(tmp.stream));
+    CU(cudaMemcpyAsync(out_keys, ok.ptr, nq * k * 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(out_dists, od.ptr, nq * k * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(out_counts, oc.ptr, nq * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
     return nullptr;
 }
 

@@ -44,10 +44,6 @@ struct join_scratch_t {
     device_buffer_t<uint64_t> iota, keys;
     device_buffer_t<float> dists, pair_out;
     device_buffer_t<uint32_t> counts, computed, visited, slot_a, slot_b;
-    ~join_scratch_t() {
-        iota.release(); keys.release(); dists.release(); pair_out.release(); counts.release(); computed.release();
-        visited.release(); slot_a.release(); slot_b.release();
-    }
 };
 
 /* the women's handle as index_gt::search sees it: every slot a candidate (no predicate), results reported as slots,
@@ -83,7 +79,7 @@ char const* frozen_index_t::join(frozen_index_t& other, size_t max_proposals, bo
     std::lock_guard<std::mutex> lock_second(second->mutex);
     if (metric != other.metric || scalar != other.scalar || dimensions != other.dimensions)
         return "Can't join indexes of different metrics, scalar kinds or dimensions";
-    if (device != other.device) return "Can't join indexes that live on different devices";
+    if (stream.device != other.stream.device) return "Can't join indexes that live on different devices";
     if (shards || other.shards) return "Can't join a sharded handle: it holds one shard of its index";
     if (max_proposals > JOIN_MAX_PROPOSALS) return "max_proposals above 65535 would overflow the per-man proposal counter";
 
@@ -125,7 +121,7 @@ char const* frozen_index_t::join(frozen_index_t& other, size_t max_proposals, bo
             size_t const nq = std::min(chunk, nm - begin);
             void const* queries = men.d.vectors + begin * vs;
             if (exact) {
-                if (char const* e = exact_search_device(women.d, women.sm_count, queries, nq, vs, k, false, true, js.keys.ptr, js.dists.ptr,
+                if (char const* e = exact_search_device(women.d, women.stream.sm_count, queries, nq, vs, k, false, true, js.keys.ptr, js.dists.ptr,
                                                         js.counts.ptr, women.exact_scratch, s))
                     return e;
                 women.kernel_launches += 2;
@@ -255,10 +251,6 @@ char const* frozen_index_t::pairwise_distances(uint64_t const* left, uint64_t co
     size_t const pairs = sa.size();
     device_buffer_t<uint32_t> d_a, d_b;
     device_buffer_t<float> d_out;
-    struct release_t {
-        device_buffer_t<uint32_t>&a, &b; device_buffer_t<float>& c;
-        ~release_t() { a.release(); b.release(); c.release(); }
-    } release{d_a, d_b, d_out};
     if (char const* e = d_a.reserve(pairs)) return e;
     if (char const* e = d_b.reserve(pairs)) return e;
     if (char const* e = d_out.reserve(pairs)) return e;

@@ -128,8 +128,6 @@ struct shard_group_t {
     device_buffer_t<uint8_t> send, recv;
     ~shard_group_t() {
         if (comm) nccl().comm_destroy(comm);
-        send.release();
-        recv.release();
     }
 };
 
@@ -221,28 +219,23 @@ char const* frozen_index_t::sharded_search_host(void const* q, size_t nq, size_t
 char const* shards_merge_host(void const* payloads, int world, size_t nq, size_t k, uint64_t* keys, float* dists, uint32_t* counts) {
     if (world < 1 || world > 32) return "Shard rank / world size out of range (1..32 shards)";
     if (!nq || !k) return nullptr;
-    frozen_index_t tmp;
-    tmp.device = default_device();
-    if (char const* e = tmp.ensure_context()) return e;
+    cuda_stream_t s(default_device());
+    if (char const* e = s.open()) return e;
     size_t const bytes = payload_bytes(nq, k);
     device_buffer_t<uint8_t> in;
     device_buffer_t<uint64_t> dk;
     device_buffer_t<float> dd;
     device_buffer_t<uint32_t> dc;
-    struct release_t {
-        device_buffer_t<uint8_t>& a; device_buffer_t<uint64_t>& b; device_buffer_t<float>& c; device_buffer_t<uint32_t>& d;
-        ~release_t() { a.release(); b.release(); c.release(); d.release(); }
-    } release{in, dk, dd, dc};
     if (char const* e = in.reserve(bytes * (size_t)world)) return e;
     if (char const* e = dk.reserve(nq * k)) return e;
     if (char const* e = dd.reserve(nq * k)) return e;
     if (char const* e = dc.reserve(nq)) return e;
-    CU(cudaMemcpyAsync(in.ptr, payloads, bytes * (size_t)world, cudaMemcpyHostToDevice, tmp.stream));
-    CU(shards_merge_launch(in.ptr, bytes, world, nq, k, dk.ptr, dd.ptr, dc.ptr, tmp.stream));
-    CU(cudaMemcpyAsync(keys, dk.ptr, nq * k * 8, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaMemcpyAsync(dists, dd.ptr, nq * k * 4, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaMemcpyAsync(counts, dc.ptr, nq * 4, cudaMemcpyDeviceToHost, tmp.stream));
-    CU(cudaStreamSynchronize(tmp.stream));
+    CU(cudaMemcpyAsync(in.ptr, payloads, bytes * (size_t)world, cudaMemcpyHostToDevice, s));
+    CU(shards_merge_launch(in.ptr, bytes, world, nq, k, dk.ptr, dd.ptr, dc.ptr, s));
+    CU(cudaMemcpyAsync(keys, dk.ptr, nq * k * 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(dists, dd.ptr, nq * k * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(counts, dc.ptr, nq * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
     return nullptr;
 }
 
