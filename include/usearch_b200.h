@@ -333,6 +333,13 @@ size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries
  * products (the tensor-core dots and their conversion; part of distance math) | cycles of the prefilter's bound (the
  * bound, its ballots and the survivors' compaction; part of distance math). */
 void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16);
+/* The same counters, the first `count` of them into `counters` (may be NULL; words beyond those the kernel keeps are
+ * zeroed). Words 0-15 are those of usearch_b200_profile_phases; then cycles of the conversion of the prefilter's dot
+ * products to `dot` and their stores, after the tensor cores have finished (part of the dot products' cycles) | the
+ * prefilter's code passes | hops measured through the prefilter | cycles of distance math in hops that start with
+ * `top` full | cycles of vector wait in the upper-level descent (part of setup+descent; distance math, which is layer-0
+ * time less every vector wait, subtracts them as well). Returns the number of counters the kernel keeps. */
+size_t usearch_b200_profile_phases_n(usearch_index_t index, int enable, uint64_t* counters, size_t count);
 /* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
  * candidates of cos / ip f32 on their int8 shadow first, on by default; "heap_head" = an upper bound on the candidate-heap
  * entries kept in shared memory, rounded down to an even number >= 2, the rest go to HBM; 0 = as planned); results never

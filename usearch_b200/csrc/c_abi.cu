@@ -654,15 +654,22 @@ void usearch_clear(usearch_index_t index, usearch_error_t*) {
     ix->release_device();
 }
 
-void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16) {
+size_t usearch_b200_profile_phases_n(usearch_index_t index, int enable, uint64_t* counters, size_t count) {
     frozen_index_t* ix = as_index(index);
     std::lock_guard<std::mutex> lock(ix->mutex);
-    if (counters16) {
-        std::memset(counters16, 0, 128);
-        if (ix->phase_cycles.ptr) cudaMemcpy(counters16, ix->phase_cycles.ptr, 128, cudaMemcpyDeviceToHost);
+    size_t const bytes = sizeof(uint64_t) * PHASE_COUNTERS;
+    if (counters && count) {
+        size_t const n = std::min<size_t>(count, PHASE_COUNTERS);
+        std::memset(counters, 0, sizeof(uint64_t) * count);
+        if (ix->phase_cycles.ptr) cudaMemcpy(counters, ix->phase_cycles.ptr, sizeof(uint64_t) * n, cudaMemcpyDeviceToHost);
     }
     ix->profile_phases = enable != 0;
-    if (ix->profile_phases && !ix->phase_cycles.reserve(16)) cudaMemset(ix->phase_cycles.ptr, 0, 128);
+    if (ix->profile_phases && !ix->phase_cycles.reserve(PHASE_COUNTERS)) cudaMemset(ix->phase_cycles.ptr, 0, bytes);
+    return PHASE_COUNTERS;
+}
+
+void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* counters16) {
+    usearch_b200_profile_phases_n(index, enable, counters16, 16);
 }
 
 int usearch_b200_tune(usearch_index_t index, char const* knob, int value) {

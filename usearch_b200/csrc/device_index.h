@@ -125,10 +125,10 @@ struct search_args_t {
      * squared norms in surv_b2) */
     uint32_t prefilter = 0, code_pass = 0, code_smem_stride = 0, off_surv_b2 = 0;
     uint32_t off_qsplit = 0, qsplit_len = 0;
-    /* optional introspection: 8 cycle counters summed over all queries (lane 0 clock64 deltas):
-     * setup+descent | heap pop | row + visited test | vector wait | distance math | accept replay | output, then counts
-     * (include/usearch_b200.h, usearch_b200_profile_phases) */
+    /* optional introspection: PHASE_COUNTERS counters summed over all queries (lane 0 clock64 deltas and counts), in
+     * the order of include/usearch_b200.h (usearch_b200_profile_phases, usearch_b200_profile_phases_n) */
     unsigned long long* phase_cycles = nullptr;
 };
+constexpr uint32_t PHASE_COUNTERS = 21;
 
 } // namespace usearch_b200

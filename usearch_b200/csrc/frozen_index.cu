@@ -601,7 +601,7 @@ char const* frozen_index_t::search_device(void const* d_queries, size_t nq, size
     a.cluster_end_level = active_cluster_end_level;
 
     if (profile_phases) {
-        if (char const* e = phase_cycles.reserve(16)) return e;
+        if (char const* e = phase_cycles.reserve(PHASE_COUNTERS)) return e;
         a.phase_cycles = phase_cycles.ptr;
     }
     CU(cudaMemsetAsync(work_counter.ptr, 0, 8, s));

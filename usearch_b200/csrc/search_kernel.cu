@@ -249,6 +249,8 @@ struct warp_ctx_t {
     uint32_t t_code;     /* introspection: cycles spent waiting for the prefilter's int8 codes */
     uint32_t t_dot;      /* introspection: the prefilter's IMMA dot products and their conversion to `dot` */
     uint32_t t_bound;    /* introspection: the prefilter's bound, ballots and compaction */
+    uint32_t t_conv;     /* introspection: the part of t_dot after the IMMAs: conversion to `dot` and its stores */
+    uint32_t n_code_pass; /* introspection: the prefilter's code passes */
 };
 
 /* ---- distances of a whole candidate list ---------------------------------------------------- */
@@ -526,11 +528,76 @@ __device__ __forceinline__ void imma_16832(int (&c)[4], uint32_t a0, uint32_t a1
                  : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
+/*
+ *  The prefilter's dot products for NT (1 or 2) tiles of 16 rows: D1 = q1.c and D2 = q2.c, exact in s32, and
+ *  `dot` = fl32(sa1 D1 + sa2 D2) into out[i] for i < cnt. NT is a template parameter so that no IMMA or ldmatrix is
+ *  predicated and no branch splits the k-loop. k outer, tiles inner: one B load per k-step serves every tile. Rows of the
+ *  last tile beyond `cnt` hold stale bytes, and the k-bytes beyond `code_stride` of a row were never copied: the split is
+ *  zero there, so they add 0 to D1 and D2, and the rows' results are dropped.
+ *  Even k-steps accumulate into acc[0], odd ones into acc[1], so that every tile has two independent chains of IMMAs; the
+ *  s32 sums are exact, so D1 and D2 do not depend on the split. Four fragment sets rotate so that the fragments of step
+ *  k + 2 are requested before the IMMAs of step k issue: no ldmatrix is consumed within two k-steps of its issue.
+ */
+template <uint32_t NT>
+__device__ __forceinline__ void prefilter_dots(uint32_t a_addr, uint32_t b_addr, uint32_t scs, uint32_t ksteps, double sa1,
+                                               double sa2, float* out, uint32_t cnt, int lane, warp_ctx_t& w, bool prof) {
+    int acc[2][NT][4] = {};
+    uint32_t f0[NT][4], f1[NT][4], f2[NT][4], f3[NT][4], b0[2], b1[2], b2[2], b3[2];
+    auto load = [&](uint32_t k, uint32_t(&A)[NT][4], uint32_t(&B)[2]) {
+        B[0] = B[1] = 0u;
+        if (lane < 8) asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(B[0]), "=r"(B[1]) : "r"(b_addr + 32u * k));
+#pragma unroll
+        for (uint32_t t = 0; t < NT; ++t) ldmatrix_x4(a_addr + t * 16u * scs + 32u * k, A[t][0], A[t][1], A[t][2], A[t][3]);
+    };
+    auto mma = [&](int (&C)[NT][4], uint32_t const(&A)[NT][4], uint32_t const(&B)[2]) {
+#pragma unroll
+        for (uint32_t t = 0; t < NT; ++t) imma_16832(C[t], A[t][0], A[t][1], A[t][2], A[t][3], B[0], B[1]);
+    };
+    static_assert(NT == 1 || NT == 2, "tiles per k-loop: 1 or 2");
+    uint32_t k = 0;
+    load(0, f0, b0);
+    if (ksteps > 1) load(1, f1, b1);
+    for (; k + 6 <= ksteps; k += 4) { /* f0, f1 hold steps k, k + 1 */
+        load(k + 2, f2, b2);
+        mma(acc[0], f0, b0);
+        load(k + 3, f3, b3);
+        mma(acc[1], f1, b1);
+        load(k + 4, f0, b0);
+        mma(acc[0], f2, b2);
+        load(k + 5, f1, b1);
+        mma(acc[1], f3, b3);
+    }
+    /* 1 to 5 steps remain, the first two of them loaded (uniform branches, once per pass) */
+    if (k + 2 < ksteps) load(k + 2, f2, b2);
+    if (k + 3 < ksteps) load(k + 3, f3, b3);
+    mma(acc[0], f0, b0);
+    if (k + 1 < ksteps) mma(acc[1], f1, b1);
+    if (k + 4 < ksteps) load(k + 4, f0, b0);
+    if (k + 2 < ksteps) mma(acc[0], f2, b2);
+    if (k + 3 < ksteps) mma(acc[1], f3, b3);
+    if (k + 4 < ksteps) mma(acc[0], f0, b0);
+    /* C: lane 4 g holds columns 0 and 1 (D1, D2) of rows g and g + 8 */
+    int d[NT][4];
+#pragma unroll
+    for (uint32_t t = 0; t < NT; ++t)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) d[t][j] = acc[0][t][j] + acc[1][t][j];
+    long long const t_conv = prof ? clock64() : 0; /* the IMMAs have retired: their sums are in registers */
+    uint32_t const g = (uint32_t)lane >> 2, sub = (uint32_t)lane & 3;
+#pragma unroll
+    for (uint32_t t = 0; t < NT; ++t) {
+        uint32_t const i = 16u * t + g;
+        if (sub == 0 && i < cnt) out[i] = __double2float_rn(sa1 * (double)d[t][0] + sa2 * (double)d[t][1]);
+        if (sub == 0 && i + 8 < cnt) out[i + 8] = __double2float_rn(sa1 * (double)d[t][2] + sa2 * (double)d[t][3]);
+    }
+    __syncwarp(); /* dots visible, and every lane is done with the stage area before it is refilled */
+    if (prof) w.t_conv += (uint32_t)(clock64() - t_conv);
+}
+
 template <class M>
 __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix, search_args_t const& a, warp_ctx_t& w,
                                                      typename M::qconst_t qc, pf_query_bound_t const& qb,
                                                      pf_query_split_t const& sp, float radius, uint32_t ncand, int lane) {
-    constexpr uint32_t MAX_TILES = 4; /* code_pass <= 64 */
     uint8_t* const smem = reinterpret_cast<uint8_t*>(w.q4); /* the query opens the warp's shared memory */
     float* const surv_b2 = reinterpret_cast<float*>(smem + a.off_surv_b2); /* cos: the survivors' stored squared norms */
     uint32_t const cs = ix.code_stride, scs = a.code_smem_stride, ksteps = a.qsplit_len / 32;
@@ -566,46 +633,18 @@ __device__ __forceinline__ uint32_t measure_prefiltered(device_index_t const& ix
             mbar_wait(bar, w.phase & 1u);
         w.phase ^= 1u;
         long long const t_dot = a.phase_cycles ? clock64() : 0;
-        /* k outer, tiles inner: one B load per k-step serves every tile. Rows of the last tile beyond `cnt` hold stale
-         * bytes, and the k-bytes beyond `code_stride` of a row were never copied: the split is zero there, so they add 0
-         * to D1 and D2, and the rows' results are dropped.
-         * Even k-steps accumulate into acc[0], odd ones into acc[1], so that every tile has two independent chains of
-         * IMMAs; the s32 sums are exact, so D1 and D2 do not depend on the split. The fragments of step k + 1 are loaded
-         * before the IMMAs of step k issue. */
+        bool const prof = a.phase_cycles != nullptr;
+        /* tiles of this pass (code_pass <= 64): 3 or 4 tiles (64-candidate passes, never at 768-d) go as two passes over
+         * the k-steps, of 2 tiles and of the rest, since the fragments of 3 or 4 tiles would push the kernel past 255
+         * registers */
         uint32_t const ntiles = (cnt + 15) / 16;
-        int acc[2][MAX_TILES][4] = {};
-        uint32_t fa[2][MAX_TILES][4], fb[2][2];
-        auto load = [&](uint32_t k, uint32_t(&A)[MAX_TILES][4], uint32_t(&B)[2]) {
-            B[0] = B[1] = 0u;
-            if (lane < 8) asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(B[0]), "=r"(B[1]) : "r"(b_addr + 32u * k));
-#pragma unroll
-            for (uint32_t t = 0; t < MAX_TILES; ++t)
-                if (t < ntiles) ldmatrix_x4(a_addr + t * 16u * scs + 32u * k, A[t][0], A[t][1], A[t][2], A[t][3]); /* uniform */
-        };
-        auto mma = [&](int (&C)[MAX_TILES][4], uint32_t const(&A)[MAX_TILES][4], uint32_t const(&B)[2]) {
-#pragma unroll
-            for (uint32_t t = 0; t < MAX_TILES; ++t)
-                if (t < ntiles) imma_16832(C[t], A[t][0], A[t][1], A[t][2], A[t][3], B[0], B[1]);
-        };
-        load(0, fa[0], fb[0]);
-        uint32_t k = 0;
-        for (; k + 2 <= ksteps; k += 2) { /* fa[0] holds step k */
-            load(k + 1, fa[1], fb[1]);
-            mma(acc[0], fa[0], fb[0]);
-            if (k + 2 < ksteps) load(k + 2, fa[0], fb[0]);
-            mma(acc[1], fa[1], fb[1]);
-        }
-        if (k < ksteps) mma(acc[0], fa[0], fb[0]); /* an odd last step */
-        /* C: lane 4 g holds columns 0 and 1 (D1, D2) of rows g and g + 8 */
-#pragma unroll
-        for (uint32_t t = 0; t < MAX_TILES; ++t) {
-            uint32_t const i = 16u * t + g;
-            int const d1 = acc[0][t][0] + acc[1][t][0], d2 = acc[0][t][1] + acc[1][t][1];
-            int const d1h = acc[0][t][2] + acc[1][t][2], d2h = acc[0][t][3] + acc[1][t][3];
-            if (sub == 0 && i < cnt) w.cand_d[base + i] = __double2float_rn(sa1 * (double)d1 + sa2 * (double)d2);
-            if (sub == 0 && i + 8 < cnt) w.cand_d[base + i + 8] = __double2float_rn(sa1 * (double)d1h + sa2 * (double)d2h);
-        }
-        __syncwarp(); /* dots visible, and every lane is done with the stage area before it is refilled */
+        if (ntiles == 1) prefilter_dots<1>(a_addr, b_addr, scs, ksteps, sa1, sa2, w.cand_d + base, cnt, lane, w, prof);
+        else prefilter_dots<2>(a_addr, b_addr, scs, ksteps, sa1, sa2, w.cand_d + base, min(cnt, 32u), lane, w, prof);
+        if (ntiles == 3)
+            prefilter_dots<1>(a_addr + 32u * scs, b_addr, scs, ksteps, sa1, sa2, w.cand_d + base + 32, cnt - 32, lane, w, prof);
+        else if (ntiles == 4)
+            prefilter_dots<2>(a_addr + 32u * scs, b_addr, scs, ksteps, sa1, sa2, w.cand_d + base + 32, cnt - 32, lane, w, prof);
+        if (prof) w.n_code_pass += 1;
         long long const t_bound = a.phase_cycles ? clock64() : 0;
         if (a.phase_cycles) w.t_dot += (uint32_t)(t_bound - t_dot);
         uint32_t const lt = (1u << lane) - 1u;
@@ -666,6 +705,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
     bool log_overflow_out = false;
     bool const prof = a.phase_cycles != nullptr;
     uint32_t pc0 = 0, pc1 = 0, pc2 = 0, pc4 = 0, pc5 = 0, n_push = 0, max_heap = 0, n_pref = 0, n_surv = 0;
+    uint32_t pc4_full = 0, n_pf_hops = 0; /* distance math of the hops that start with `top` full; prefiltered hops */
     /* the layer-0 prefilter: plain searches of the f32 metrics that declare it, on an index that has the shadow */
     constexpr bool PF = prefilter_of<M>::value && STAGED && !INSERT;
     long long tp = prof ? clock64() : 0;
@@ -673,6 +713,8 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
     w.t_code = 0;
     w.t_dot = 0;
     w.t_bound = 0;
+    w.t_conv = 0;
+    w.n_code_pass = 0;
 #define PHASE(acc)                                  \
     if (prof) {                                     \
         long long now_ = clock64();                 \
@@ -785,6 +827,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
             } while (changed);
         }
 
+        if (prof && lane == 0) atomicAdd(a.phase_cycles + 20, (unsigned long long)w.t_wait); /* the descent's vector waits */
         /* ---- search_to_find_in_base_ (index.hpp:4175-4246) ---- */
         if (lane == 0) cand_s[0] = closest;
         __syncwarp();
@@ -941,17 +984,20 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
 
             bool measured = false;
             uint32_t nacc = ncand; /* the candidates the accept replay visits */
+            uint32_t const waits0 = w.t_wait + w.t_code, pc4_0 = pc4; /* introspection */
             if constexpr (PF) {
                 if (a.prefilter && top_size == ef) { /* `top` full: every candidate must beat the radius */
                     nacc = measure_prefiltered<M>(ix, a, w, qc, pf_qb, pf_sp, radius, ncand, lane);
                     n_pref += ncand;
                     n_surv += nacc;
+                    n_pf_hops += 1;
                     measured = true;
                 }
             }
             if (!measured) measure_list<M, STAGED>(ix, a, w, qc, ncand, lane);
             computed += ncand;
             PHASE(pc4)
+            if (prof && top_size == ef) pc4_full += (pc4 - pc4_0) - (w.t_wait + w.t_code - waits0);
 
             /* The reference's sequential accept loop, replayed in stored order. `radius` only shrinks
              * and `top` only grows inside a hop, so a candidate that fails `|top|<ef || d<radius` at the
@@ -1074,6 +1120,10 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         atomicAdd(a.phase_cycles + 13, (unsigned long long)w.t_code);
         atomicAdd(a.phase_cycles + 14, (unsigned long long)w.t_dot);
         atomicAdd(a.phase_cycles + 15, (unsigned long long)w.t_bound);
+        atomicAdd(a.phase_cycles + 16, (unsigned long long)w.t_conv);
+        atomicAdd(a.phase_cycles + 17, (unsigned long long)w.n_code_pass);
+        atomicAdd(a.phase_cycles + 18, (unsigned long long)n_pf_hops);
+        atomicAdd(a.phase_cycles + 19, (unsigned long long)pc4_full);
     }
 #undef PHASE
 }

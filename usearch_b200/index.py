@@ -49,7 +49,7 @@ EXPORTED_SYMBOLS = [
     # additive
     "usearch_search_many", "usearch_b200_search_many_device", "usearch_b200_search_many_stats",
     "usearch_b200_filtered_search_many", "usearch_b200_exact_search_many", "usearch_b200_cluster_many",
-    "usearch_b200_profile_phases", "usearch_b200_device", "usearch_b200_kernel_launches", "usearch_b200_last_kernel_ms",
+    "usearch_b200_profile_phases", "usearch_b200_profile_phases_n", "usearch_b200_device", "usearch_b200_kernel_launches", "usearch_b200_last_kernel_ms",
     "usearch_b200_bytes_per_vector", "usearch_b200_max_level", "usearch_b200_add_many", "usearch_b200_add_many_device",
     "usearch_b200_shards_unique_id", "usearch_b200_shards_join", "usearch_b200_sharded_search_many",
     "usearch_b200_sharded_search_many_device", "usearch_b200_shards_payload_bytes", "usearch_b200_merge_topk",
@@ -128,6 +128,8 @@ def load_library() -> C.CDLL:
                                          C.c_size_t, C.c_int, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                          C.c_size_t, err]
     lib.usearch_b200_profile_phases.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    lib.usearch_b200_profile_phases_n.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
+    lib.usearch_b200_profile_phases_n.restype = C.c_size_t
     lib.usearch_b200_device.argtypes = [C.c_void_p]
     lib.usearch_b200_kernel_launches.restype = C.c_uint64
     lib.usearch_b200_kernel_launches.argtypes = [C.c_void_p]
@@ -642,8 +644,8 @@ class Index:
 
     def profile_phases(self, enable: bool = True) -> dict:
         """Read (then reset) the kernel's per-phase cycle counters; see include/usearch_b200.h."""
-        out = np.zeros(16, dtype=np.uint64)
-        self._lib.usearch_b200_profile_phases(self._h, int(enable), out.ctypes.data_as(C.c_void_p))
+        out = np.zeros(21, dtype=np.uint64)
+        self._lib.usearch_b200_profile_phases_n(self._h, int(enable), out.ctypes.data_as(C.c_void_p), out.size)
         names = ["setup_descent", "heap_pop", "row_visited", "vector_wait", "distance_math", "accept", "output"]
         q = max(int(out[7]), 1)
         return {"queries": int(out[7]), **{n: float(out[i]) / q for i, n in enumerate(names)},
@@ -652,7 +654,16 @@ class Index:
                 "prefilter_dot": float(out[14]) / q, "prefilter_bound": float(out[15]) / q,
                 # what distance_math holds besides the prefilter: the survivors' FFMA pass and `finalize`, and whole
                 # lists measured without it (hops before `top` is full)
-                "survivor_math": float(out[4] - out[14] - out[15]) / q}
+                "survivor_math": float(out[4] - out[14] - out[15]) / q,
+                # the part of prefilter_dot after the tensor cores: the conversion to `dot` and its stores
+                "prefilter_convert": float(out[16]) / q,
+                "code_passes_per_prefiltered_hop": float(out[17]) / max(int(out[18]), 1),
+                "prefiltered_hops": float(out[18]) / q,
+                # distance_math split: hops that start with `top` full, and the rest (whole lists: the layer-0 hops before
+                # `top` fills). distance_math also subtracts the descent's vector waits, which belong to setup_descent.
+                "distance_math_full": float(out[19]) / q,
+                "distance_math_rest": (float(out[4]) + float(out[20]) - float(out[19])) / q,
+                "descent_vector_wait": float(out[20]) / q}
 
     # ---- sharded search: this index is one shard of a group of processes (shards.cu) ------------------------
     def join_shards(self, rank: int, world: int, unique_id: bytes) -> None:
