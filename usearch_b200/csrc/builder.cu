@@ -37,6 +37,7 @@
 #include "cuda_check.h"
 #include "frozen_index.h"
 #include "metrics.cuh"
+#include "scalar_casts.h"
 #include "warp_primitives.cuh"
 
 namespace usearch_b200 {
@@ -470,25 +471,31 @@ cudaError_t launch_pairs(device_index_t const& ix, device_index_t const& b, uint
     BUILD_DISPATCH(launch_pairs_t, ix, b, slot_a, slot_b, n, out, s)
 }
 
-/* ---- scalar casts on the device (index_plugins.hpp:1105-1224) --------------------------------------------------------- */
-
-__device__ __forceinline__ uint16_t f32_to_bf16_bits(float f) { /* simsimd_f32_to_bf16: round to nearest even, quiet NaNs */
-    uint32_t x = __float_as_uint(f);
-    if ((x & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((x >> 16) | 0x40u);
-    x += 0x7FFFu + ((x >> 16) & 1u);
-    return (uint16_t)(x >> 16);
-}
+/* ---- scalar casts on the device (index_plugins.hpp:1105-1224; the element conversions are scalar_casts.h) ------------- */
 
 /* element i of a row in scalar kind `kind`, as the value the reference's cast_gt<from, *> sees */
 __device__ __forceinline__ double load_scalar(uint8_t const* row, uint32_t kind, uint32_t i) {
     switch (kind) {
     case SCALAR_F32: return (double)reinterpret_cast<float const*>(row)[i];
     case SCALAR_F64: return reinterpret_cast<double const*>(row)[i];
-    case SCALAR_F16: return (double)__half2float(reinterpret_cast<__half const*>(row)[i]);
-    case SCALAR_BF16: return (double)__uint_as_float((uint32_t)reinterpret_cast<uint16_t const*>(row)[i] << 16);
+    case SCALAR_F16: return (double)f16_bits_to_f32(reinterpret_cast<uint16_t const*>(row)[i]);
+    case SCALAR_BF16: return (double)bf16_bits_to_f32(reinterpret_cast<uint16_t const*>(row)[i]);
     case SCALAR_I8: return (double)((float)reinterpret_cast<int8_t const*>(row)[i] / 127.f); /* cast_from_i8_gt */
     case SCALAR_B1: return (row[i >> 3] & (128u >> (i & 7u))) ? 1.0 : 0.0;                   /* cast_from_b1x8_gt */
     default: return 0.0;
+    }
+}
+
+/* the same element as an f32, for f32 / f16 / bf16 targets: an f32 source is read as it is and an f64 narrowed as the host
+ * narrows it, so that NaN payloads and signalling NaNs reach the half casts unchanged (an f64 round trip would quiet
+ * them, and the device's own f64 -> f32 conversion returns a canonical NaN) */
+__device__ __forceinline__ float load_f32(uint8_t const* row, uint32_t kind, uint32_t i) {
+    switch (kind) {
+    case SCALAR_F32: return reinterpret_cast<float const*>(row)[i];
+    case SCALAR_F64: return f64_to_f32(reinterpret_cast<double const*>(row)[i]);
+    case SCALAR_F16: return f16_bits_to_f32(reinterpret_cast<uint16_t const*>(row)[i]);
+    case SCALAR_BF16: return bf16_bits_to_f32(reinterpret_cast<uint16_t const*>(row)[i]);
+    default: return (float)load_scalar(row, kind, i); /* i8 and b1 values are finite */
     }
 }
 
@@ -510,10 +517,11 @@ __global__ void cast_elements_kernel(uint8_t const* src, size_t src_stride, uint
         return;
     }
     /* f64 sources are narrowed to f32 first: f16_bits_t(double) / bf16_bits_t(double), index_plugins.hpp:489, :553 */
-    float const v = (float)load_scalar(in, from, i);
+    float const v = load_f32(in, from, i);
     if (to == SCALAR_F32) reinterpret_cast<float*>(out)[i] = v;
-    else if (to == SCALAR_F16) reinterpret_cast<__half*>(out)[i] = __float2half_rn(v);
+    else if (to == SCALAR_F16) reinterpret_cast<uint16_t*>(out)[i] = f32_to_f16_bits(v);
     else if (to == SCALAR_BF16) reinterpret_cast<uint16_t*>(out)[i] = f32_to_bf16_bits(v);
+    else if (to == SCALAR_I8) reinterpret_cast<int8_t*>(out)[i] = v > 0 ? 1 : 0; /* b1 sources only: cast_from_b1x8_gt<i8_t> */
 }
 
 /* cast_to_i8_gt (index_plugins.hpp:1172-1191): x * 127 / |x| in f64, clamp, truncate; the magnitude is the SEQUENTIAL f64
@@ -626,11 +634,11 @@ char const* cast_rows_device(uint8_t const* src, size_t src_stride, uint32_t fro
         return nullptr;
     }
     if (!bits_per_scalar(from)) return "Unknown scalar kind!";
-    if (to == SCALAR_I8) {
+    if (to == SCALAR_I8 && from != SCALAR_B1) {
         cast_rows_to_i8_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, s>>>(src, src_stride, from, dst, dst_stride, (uint32_t)dims, rows);
     } else if (to == SCALAR_F64) {
         cast_elements_to_f64_kernel<<<(unsigned)((rows * dims + 255) / 256), 256, 0, s>>>(src, src_stride, from, dst, dst_stride, (uint32_t)dims, rows);
-    } else if (to == SCALAR_F32 || to == SCALAR_F16 || to == SCALAR_BF16 || to == SCALAR_B1) {
+    } else if (to == SCALAR_F32 || to == SCALAR_F16 || to == SCALAR_BF16 || to == SCALAR_B1 || to == SCALAR_I8) {
         size_t const total = rows * (to == SCALAR_B1 ? (dims + 7) / 8 : dims);
         cast_elements_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(src, src_stride, from, dst, dst_stride, to, (uint32_t)dims, rows);
     } else

@@ -11,9 +11,9 @@
  *    index_plugins.hpp:1105-1224 query casts
  */
 #include "cuda_check.h"
-#include "f64_casts.h"
 #include "frozen_index.h"
 #include "prefilter_bound.h"
+#include "scalar_casts.h"
 
 #include <algorithm>
 #include <cmath>
@@ -678,91 +678,6 @@ char const* frozen_index_t::retry_overflowed(search_args_t const& a, bool maxed,
 }
 
 /* ---------------------------------------------------------------------------------------------- */
-/*  host-side casts                                                                               */
-/* ---------------------------------------------------------------------------------------------- */
-
-namespace {
-
-uint16_t f32_to_f16_rn(float f) {
-    uint32_t x;
-    std::memcpy(&x, &f, 4);
-    uint32_t sign = (x >> 16) & 0x8000u;
-    uint32_t mant = x & 0x7FFFFFu;
-    int32_t exp = (int32_t)((x >> 23) & 0xFF);
-    if (exp == 255) return (uint16_t)(sign | 0x7C00u | (mant ? 0x200u | (mant >> 13) : 0));
-    exp = exp - 127 + 15;
-    if (exp >= 31) return (uint16_t)(sign | 0x7C00u);
-    if (exp <= 0) {
-        if (exp < -10) return (uint16_t)sign;
-        mant |= 0x800000u;
-        uint32_t shift = (uint32_t)(14 - exp);
-        uint32_t half = mant >> shift;
-        uint32_t rem = mant & ((1u << shift) - 1), mid = 1u << (shift - 1);
-        if (rem > mid || (rem == mid && (half & 1))) ++half;
-        return (uint16_t)(sign | half);
-    }
-    uint32_t half = ((uint32_t)exp << 10) | (mant >> 13);
-    uint32_t rem = mant & 0x1FFFu;
-    if (rem > 0x1000u || (rem == 0x1000u && (half & 1))) ++half;
-    return (uint16_t)(sign | half);
-}
-
-uint16_t f32_to_bf16_rn(float f) {
-    uint32_t x;
-    std::memcpy(&x, &f, 4);
-    if ((x & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((x >> 16) | 0x40u);
-    x += 0x7FFFu + ((x >> 16) & 1u);
-    return (uint16_t)(x >> 16);
-}
-
-} // namespace
-
-char const* cast_queries(uint32_t from, uint32_t to, size_t dims, uint8_t const* src, size_t src_stride, size_t nq,
-                         uint8_t* dst, size_t dst_stride) {
-    size_t const to_bytes = (dims * bits_per_scalar(to) + 7) / 8;
-    if (from == to) {
-        for (size_t i = 0; i < nq; ++i) std::memcpy(dst + i * dst_stride, src + i * src_stride, to_bytes);
-        return nullptr;
-    }
-    if (from != SCALAR_F32 && from != SCALAR_F64) return "Only f32/f64 queries can be cast to the index's scalar kind";
-    std::vector<float> row(dims);
-    for (size_t i = 0; i < nq; ++i) {
-        uint8_t const* s = src + i * src_stride;
-        uint8_t* o = dst + i * dst_stride;
-        if (from == SCALAR_F32) std::memcpy(row.data(), s, dims * 4);
-        else
-            for (size_t j = 0; j < dims; ++j) { double v; std::memcpy(&v, s + j * 8, 8); row[j] = (float)v; }
-        switch (to) {
-        case SCALAR_F32: std::memcpy(o, row.data(), dims * 4); break;
-        case SCALAR_F16:
-            for (size_t j = 0; j < dims; ++j) { uint16_t h = f32_to_f16_rn(row[j]); std::memcpy(o + 2 * j, &h, 2); }
-            break;
-        case SCALAR_BF16:
-            for (size_t j = 0; j < dims; ++j) { uint16_t h = f32_to_bf16_rn(row[j]); std::memcpy(o + 2 * j, &h, 2); }
-            break;
-        case SCALAR_I8: { /* cast_to_i8_gt, index_plugins.hpp:1172-1191 */
-            double magnitude = 0;
-            for (size_t j = 0; j < dims; ++j) magnitude += (double)row[j] * (double)row[j];
-            magnitude = std::sqrt(magnitude);
-            for (size_t j = 0; j < dims; ++j) {
-                double v = row[j] * 127.0 / magnitude;
-                v = v > 127.0 ? 127.0 : (v < -127.0 ? -127.0 : v);
-                reinterpret_cast<int8_t*>(o)[j] = (int8_t)v;
-            }
-            break;
-        }
-        case SCALAR_B1: /* cast_to_b1x8_gt, index_plugins.hpp:1139-1158 */
-            std::memset(o, 0, to_bytes);
-            for (size_t j = 0; j < dims; ++j)
-                if (row[j] > 0) o[j / 8] |= (uint8_t)(128 >> (j & 7));
-            break;
-        default: return "Unsupported scalar kind";
-        }
-    }
-    return nullptr;
-}
-
-/* ---------------------------------------------------------------------------------------------- */
 /*  batched search on host buffers: H2D + kernel + D2H inside the call                            */
 /* ---------------------------------------------------------------------------------------------- */
 
@@ -1050,59 +965,6 @@ char const* frozen_index_t::rename_key(uint64_t from, uint64_t to, size_t* renam
     return nullptr;
 }
 
-namespace {
-
-float half_bits_to_f32(uint16_t h) {
-    uint32_t const sign = (uint32_t)(h & 0x8000u) << 16, exp = (h >> 10) & 0x1Fu, mant = h & 0x3FFu;
-    uint32_t bits;
-    if (exp == 0) {
-        if (!mant) bits = sign;
-        else { /* subnormal: renormalise */
-            int e = -1;
-            uint32_t m = mant;
-            do { ++e; m <<= 1; } while (!(m & 0x400u));
-            bits = sign | ((uint32_t)(127 - 15 - e) << 23) | ((m & 0x3FFu) << 13);
-        }
-    } else if (exp == 31) bits = sign | 0x7F800000u | (mant << 13);
-    else bits = sign | ((exp + 112u) << 23) | (mant << 13);
-    float f;
-    std::memcpy(&f, &bits, 4);
-    return f;
-}
-
-/* one stored vector -> the caller's scalar kind (index_dense_gt::get_ casts with casts_.to_*, index_dense.hpp:2121-2150) */
-char const* cast_stored_row(uint32_t from, uint32_t to, size_t dims, uint8_t const* src, uint8_t* dst) {
-    size_t const to_bytes = (dims * bits_per_scalar(to) + 7) / 8;
-    if (from == to) { std::memcpy(dst, src, to_bytes); return nullptr; }
-    if (from == SCALAR_F64) { /* cast_gt<f64, *>: i8 and b1 read the doubles, the rest narrow to f32 first */
-        std::vector<double> x(dims);
-        std::memcpy(x.data(), src, dims * 8);
-        if (to == SCALAR_I8) { cast_f64_to_i8(x.data(), dims, reinterpret_cast<int8_t*>(dst)); return nullptr; }
-        if (to == SCALAR_B1) { cast_f64_to_b1(x.data(), dims, dst); return nullptr; }
-        std::vector<float> row(dims);
-        for (size_t j = 0; j < dims; ++j) row[j] = (float)x[j];
-        return cast_queries(SCALAR_F32, to, dims, reinterpret_cast<uint8_t const*>(row.data()), dims * 4, 1, dst, to_bytes);
-    }
-    std::vector<float> row(dims);
-    for (size_t j = 0; j < dims; ++j) {
-        switch (from) {
-        case SCALAR_F32: std::memcpy(&row[j], src + 4 * j, 4); break;
-        case SCALAR_F16: { uint16_t h; std::memcpy(&h, src + 2 * j, 2); row[j] = half_bits_to_f32(h); break; }
-        case SCALAR_BF16: { uint16_t h; std::memcpy(&h, src + 2 * j, 2); uint32_t b = (uint32_t)h << 16; std::memcpy(&row[j], &b, 4); break; }
-        case SCALAR_I8: row[j] = (float)reinterpret_cast<int8_t const*>(src)[j] / 127.f; break;     /* cast_from_i8_gt */
-        case SCALAR_B1: row[j] = (src[j >> 3] & (128u >> (j & 7u))) ? 1.f : 0.f; break;            /* cast_from_b1x8_gt */
-        default: return "Unsupported scalar kind";
-        }
-    }
-    if (to == SCALAR_F64) {
-        for (size_t j = 0; j < dims; ++j) { double v = row[j]; std::memcpy(dst + 8 * j, &v, 8); }
-        return nullptr;
-    }
-    return cast_queries(SCALAR_F32, to, dims, reinterpret_cast<uint8_t const*>(row.data()), dims * 4, 1, dst, to_bytes);
-}
-
-} // namespace
-
 /* index_dense_gt::get (index_dense.hpp:781-786 -> get_ :2121-2150): up to `max_count` vectors stored under `key` */
 char const* frozen_index_t::get_vectors(uint64_t key, size_t max_count, void* out, uint32_t out_scalar, size_t* found) {
     *found = 0;
@@ -1117,7 +979,8 @@ char const* frozen_index_t::get_vectors(uint64_t key, size_t max_count, void* ou
     std::vector<uint8_t> row(d.vec_stride);
     for (size_t i = 0; i < slots.size(); ++i) {
         CU(cudaMemcpy(row.data(), d.vectors + (size_t)slots[i] * d.vec_stride, d.bytes_per_vector, cudaMemcpyDeviceToHost));
-        if (char const* e = cast_stored_row(scalar, out_scalar, dimensions, row.data(), static_cast<uint8_t*>(out) + i * out_bytes)) return e;
+        /* index_dense_gt::get_ casts with casts_.to_* (index_dense.hpp:2121-2150) */
+        if (char const* e = cast_row_host(scalar, out_scalar, dimensions, row.data(), static_cast<uint8_t*>(out) + i * out_bytes)) return e;
     }
     *found = slots.size();
     return nullptr;

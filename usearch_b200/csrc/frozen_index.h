@@ -269,9 +269,6 @@ char const* iota_u64_device(uint64_t* d_out, size_t n, cudaStream_t stream);
 char const* pair_distance_host(void const* a, void const* b, uint32_t scalar, size_t dimensions, uint32_t metric, float* result);
 int default_device(); /* USEARCH_B200_DEVICE, else LOCAL_RANK (one process per GPU under torchrun), else 0 */
 
-/* host-side query casts (index_plugins.hpp:1105-1224) */
-char const* cast_queries(uint32_t from_scalar, uint32_t to_scalar, size_t dims, uint8_t const* src, size_t src_stride, size_t nq,
-                         uint8_t* dst, size_t dst_stride);
 size_t bits_per_scalar(uint32_t scalar);
 
 } // namespace usearch_b200
