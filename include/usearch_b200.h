@@ -209,6 +209,36 @@ void usearch_b200_last_join_ms(usearch_index_t index, float* out3);
 void usearch_b200_pairwise_distances(usearch_index_t index, usearch_key_t const* left_keys, usearch_key_t const* right_keys, size_t n,
                                      usearch_distance_t* out, usearch_error_t* error);
 
+/* ---- additive: reading the index back out (index_dense_gt's get / export_keys / copy / stats) ---------------------- */
+
+/* NEW (additive). index_dense_gt::get for `count` keys in one call (python/lib.cpp:971-1003). Each key gets
+ * min(usearch_count(key), max_per_key) rows, in ascending slot order (the rows usearch_get would give). The rows are
+ * packed in key order into `vectors`, `vectors_stride` bytes apart (0 = dense), cast to `kind` with the rules of
+ * usearch_get. A key that is missing gets no row. `counts[i]` receives the rows of key i. Returns the number of rows.
+ * The slots are resolved on the host; one gather kernel, a cast kernel when `kind` differs from the stored kind, and one
+ * copy back run per chunk of rows, and the device and pinned scratch stay bounded (the "get_chunk_rows" knob). */
+size_t usearch_b200_get_many(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t max_per_key, void* vectors,
+                             size_t vectors_stride, usearch_scalar_kind_t kind, size_t* counts, usearch_error_t* error);
+/* NEW (additive). index_dense_gt::export_keys (index_dense.hpp:1595-1608): the live keys from the `offset`-th on, at most
+ * `limit` of them, in ascending slot order (the reference walks its hash table instead). Returns the number written. */
+size_t usearch_b200_export_keys(usearch_index_t index, size_t offset, size_t limit, usearch_key_t* keys, usearch_error_t* error);
+/* keys[i] = the offsets[i]-th live key in the same order, for `count` offsets in any order; an offset past the last live
+ * key is an error */
+void usearch_b200_export_keys_at(usearch_index_t index, size_t const* offsets, size_t count, usearch_key_t* keys,
+                                 usearch_error_t* error);
+/* NEW (additive). index_dense_gt::copy (index_dense.hpp:1615-1650): a new, independent handle on the same device holding
+ * a copy of every array and of all host state (configuration, free-slot queue, knobs). Free it with usearch_free. The
+ * same further calls on both give identical results and identical files. A sharded handle is refused. */
+usearch_index_t usearch_b200_copy(usearch_index_t index, usearch_error_t* error);
+/* NEW (additive). index_gt::stats (index.hpp:3133-3225). `per_level4` receives, for each level 0 .. max_level (at most
+ * `levels_capacity` of them), nodes | edges | max_edges | allocated_bytes as stats(stats_per_level, max_level) gives
+ * them; `total4` (may be NULL) receives stats(). Edges are the entries the device lists hold, counted in one launch;
+ * allocated_bytes follows the reference's node layout, not HBM use. Returns max_level + 1, or 0 for an empty index. */
+size_t usearch_b200_levels_stats(usearch_index_t index, size_t* per_level4, size_t levels_capacity, size_t* total4,
+                                 usearch_error_t* error);
+/* Whether the index keeps several entries per key. */
+bool usearch_b200_multi(usearch_index_t index);
+
 /* ---- additive: sharded search, one process per GPU (SURVEY.md §8e) ------------------------------------------------ */
 
 /* The reference's `Indexes` (python/lib.cpp:74-107, :321-402) searches every query in every shard and merges by distance. Here
@@ -342,8 +372,9 @@ void usearch_b200_profile_phases(usearch_index_t index, int enable, uint64_t* co
 size_t usearch_b200_profile_phases_n(usearch_index_t index, int enable, uint64_t* counters, size_t count);
 /* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
  * candidates of cos / ip f32 on their int8 shadow first, on by default; "heap_head" = an upper bound on the candidate-heap
- * entries kept in shared memory, rounded down to an even number >= 2, the rest go to HBM; 0 = as planned); results never
- * depend on them. Returns 0, or -1 for an unknown knob. */
+ * entries kept in shared memory, rounded down to an even number >= 2, the rest go to HBM; 0 = as planned), and
+ * "get_chunk_rows" = rows per chunk of usearch_b200_get_many (0 = 64 MB of output); results never depend on them.
+ * Returns 0, or -1 for an unknown knob. */
 int usearch_b200_tune(usearch_index_t index, char const* knob, int value);
 /* The launch plan a search of `count` neighbours gets under the current knobs, for a loaded index. `out16` receives:
  * stage sets | warps per SM (target) | blocks | shared memory per warp (bytes) | heap entries in shared memory | heap

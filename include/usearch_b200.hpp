@@ -263,6 +263,54 @@ class index_dense_t {
         usearch_error_t error = nullptr;
         return usearch_get(handle_, key, vectors_limit, vectors, scalar_kind<scalar_at>(), &error);
     }
+    /* get for `count` keys in one call: up to `vectors_per_key` rows per key, packed in key order into `vectors`, with
+     * counts[i] the rows of key i (may be NULL); returns the number of rows */
+    template <typename scalar_at>
+    std::size_t get(vector_key_t const* keys, std::size_t count, scalar_at* vectors, std::size_t* counts,
+                    std::size_t vectors_per_key = 1) const {
+        std::vector<std::size_t> own(counts ? 0 : count);
+        usearch_error_t error = nullptr;
+        return usearch_b200_get_many(handle_, keys, count, vectors_per_key, vectors, 0, scalar_kind<scalar_at>(),
+                                     counts ? counts : own.data(), &error);
+    }
+    /* index_dense.hpp:1595-1608, the live keys in slot order */
+    void export_keys(vector_key_t* keys, std::size_t offset, std::size_t limit) const {
+        usearch_b200_export_keys(handle_, offset, limit, keys, nullptr);
+    }
+    bool multi() const { return usearch_b200_multi(handle_); }
+    /* index_dense.hpp:1615-1650: an independent index with the same contents */
+    state_result_t copy() const;
+
+    /* stats_t and the three stats functions of index_gt (index.hpp:3133-3225) */
+    struct stats_t {
+        std::size_t nodes = 0, edges = 0, max_edges = 0, allocated_bytes = 0;
+    };
+    stats_t stats() const {
+        stats_t total;
+        usearch_b200_levels_stats(handle_, nullptr, 0, &total.nodes, nullptr);
+        return total;
+    }
+    /* levels 0 .. max_level into stats_per_level, the head of a node counted on level 0 only; returns their sum */
+    stats_t stats(stats_t* stats_per_level, std::size_t max_level) const {
+        std::vector<stats_t> levels(usearch_b200_levels_stats(handle_, nullptr, 0, nullptr, nullptr));
+        usearch_b200_levels_stats(handle_, &levels.data()->nodes, levels.size(), nullptr, nullptr);
+        stats_t total;
+        for (std::size_t l = 0; l <= max_level; ++l) {
+            stats_t const s = l < levels.size() ? levels[l] : stats_t();
+            stats_per_level[l] = s;
+            total.nodes += s.nodes, total.edges += s.edges, total.max_edges += s.max_edges, total.allocated_bytes += s.allocated_bytes;
+        }
+        return total;
+    }
+    /* the nodes on `level` and above, the 10-byte head of a node (key and level) counted on every level */
+    stats_t stats(std::size_t level) const {
+        std::vector<stats_t> levels(level + 1);
+        stats(levels.data(), level);
+        stats_t s = levels[level];
+        if (level) s.allocated_bytes += 10 * s.nodes;
+        return s;
+    }
+
     labeling_result_t remove(vector_key_t key) {
         labeling_result_t result;
         usearch_error_t error = nullptr;
@@ -369,6 +417,14 @@ inline index_dense_t::state_result_t index_dense_t::make(metric_punned_t metric,
     options.multi = config.multi;
     usearch_error_t error = nullptr;
     state.index.handle_ = usearch_init(&options, &error);
+    state.error = error;
+    return state;
+}
+
+inline index_dense_t::state_result_t index_dense_t::copy() const {
+    state_result_t state;
+    usearch_error_t error = nullptr;
+    state.index.handle_ = usearch_b200_copy(handle_, &error);
     state.error = error;
     return state;
 }

@@ -437,6 +437,87 @@ size_t usearch_get(usearch_index_t index, usearch_key_t key, size_t count, void*
     return found;
 }
 
+size_t usearch_b200_get_many(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t max_per_key, void* vectors,
+                             size_t vectors_stride, usearch_scalar_kind_t kind, size_t* counts, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    uint32_t const vs = scalar_to_char(kind);
+    if (!vs) { set_error(error, "Unknown scalar kind!"); return 0; }
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    size_t rows = 0;
+    set_error(error, guarded([&] { return ix->get_many(keys, count, max_per_key, vectors, vectors_stride, vs, counts, &rows); }));
+    return rows;
+}
+
+size_t usearch_b200_export_keys(usearch_index_t index, size_t offset, size_t limit, usearch_key_t* keys, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    size_t written = 0;
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        written = ix->export_keys(offset, limit, keys);
+        return nullptr;
+    }));
+    return written;
+}
+
+void usearch_b200_export_keys_at(usearch_index_t index, size_t const* offsets, size_t count, usearch_key_t* keys, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        return ix->export_keys_at(offsets, count, keys);
+    }));
+}
+
+usearch_index_t usearch_b200_copy(usearch_index_t index, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    frozen_index_t* copy = nullptr;
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    char const* e = guarded([&]() -> char const* {
+        copy = new frozen_index_t();
+        return ix->copy_into(*copy);
+    });
+    if (e) {
+        delete copy;
+        set_error(error, e);
+        return nullptr;
+    }
+    return copy;
+}
+
+size_t usearch_b200_levels_stats(usearch_index_t index, size_t* per_level4, size_t levels_capacity, size_t* total4, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    std::vector<uint64_t> nodes, edges;
+    if (char const* e = guarded([&] { return ix->graph_levels(nodes, edges); })) {
+        set_error(error, e);
+        return 0;
+    }
+    /* node_bytes_ (index.hpp:2116-2195): a 10-byte head (key, level), then {u32 count, M0 slots} and {u32 count, M slots} per
+     * upper level */
+    size_t const m = ix->connectivity, m0 = ix->connectivity_base, head = 10, nb = 4 + 4 * m, nb0 = 4 + 4 * m0;
+    size_t total[4] = {0, 0, 0, 0};
+    for (size_t l = 0; l < nodes.size(); ++l) { /* stats(): every level of every node */
+        total[0] = l ? total[0] : nodes[0];
+        total[1] += edges[l];
+        total[2] += nodes[l] * (l ? m : m0);
+        total[3] += nodes[l] * (l ? nb : nb0 + head);
+    }
+    if (total4) std::memcpy(total4, total, sizeof(total));
+    /* stats(stats_per_level, max_level): levels 0 .. max_level, the head counted on level 0 only */
+    size_t const levels = nodes.empty() ? 0 : (size_t)ix->d.max_level + 1;
+    for (size_t l = 0; l < std::min(levels, levels_capacity); ++l) {
+        size_t const nl = l < nodes.size() ? nodes[l] : 0;
+        per_level4[4 * l + 0] = nl;
+        per_level4[4 * l + 1] = l < edges.size() ? edges[l] : 0;
+        per_level4[4 * l + 2] = nl * (l ? m : m0);
+        per_level4[4 * l + 3] = nl * (l ? nb : nb0 + head);
+    }
+    return levels;
+}
+
+bool usearch_b200_multi(usearch_index_t index) { return as_index(index)->multi; }
+
 size_t usearch_remove(usearch_index_t index, usearch_key_t key, usearch_error_t* error) { /* c/lib.cpp:439-446 */
     return usearch_b200_remove_many(index, &key, 1, false, nullptr, error);
 }
@@ -679,6 +760,7 @@ int usearch_b200_tune(usearch_index_t index, char const* knob, int value) {
     else if (!std::strcmp(knob, "warps_per_sm")) ix->tune.warps_per_sm = value;
     else if (!std::strcmp(knob, "prefilter")) ix->tune.prefilter = value;
     else if (!std::strcmp(knob, "heap_head")) ix->tune.heap_head = value;
+    else if (!std::strcmp(knob, "get_chunk_rows")) ix->tune.get_chunk_rows = value;
     else return -1;
     return 0;
 }

@@ -121,6 +121,7 @@ struct frozen_index_t {
         int prefilter = env_int("USEARCH_B200_PREFILTER", 1);       /* 0 = measure every layer-0 candidate exactly */
         int heap_head = env_int("USEARCH_B200_HEAP_HEAD", 0);       /* 0 = as planned, else an upper bound on the heap
                                                                        entries kept in shared memory (even, >= 2) */
+        int get_chunk_rows = env_int("USEARCH_B200_GET_CHUNK_ROWS", 0); /* rows per chunk of get_many; 0 = 64 MB of output */
         static int env_int(char const* name, int fallback) {
             char const* v = std::getenv(name);
             return v ? std::atoi(v) : fallback;
@@ -178,6 +179,14 @@ struct frozen_index_t {
     char const* isolate(size_t* pruned);
     char const* rename_key(uint64_t from, uint64_t to, size_t* renamed);
     char const* get_vectors(uint64_t key, size_t max_count, void* out, uint32_t out_scalar, size_t* found);
+
+    /* surface.cu: reading the index back out */
+    char const* get_many(uint64_t const* keys, size_t n, size_t max_per_key, void* out, size_t out_stride, uint32_t out_scalar,
+                         size_t* counts, size_t* rows);
+    size_t export_keys(size_t offset, size_t limit, uint64_t* out) const;
+    char const* export_keys_at(size_t const* offsets, size_t n, uint64_t* out) const;
+    char const* copy_into(frozen_index_t& copy);
+    char const* graph_levels(std::vector<uint64_t>& nodes, std::vector<uint64_t>& edges);
 
     /* join.cu: the reference's stable-marriage `join` of this index (a) with `other` (b), replayed as its one-thread run.
      * Pairs (a key, b key) come out in the reference's export order; stats as join_result_t. */

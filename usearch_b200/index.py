@@ -58,6 +58,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_reuse_removed", "usearch_b200_join", "usearch_b200_pairwise_distances",
     "usearch_b200_last_join_ms", "usearch_b200_indexes_init", "usearch_b200_indexes_free", "usearch_b200_indexes_merge",
     "usearch_b200_indexes_size", "usearch_b200_indexes_search_many", "usearch_b200_indexes_last_ms", "usearch_b200_merge_into",
+    "usearch_b200_get_many", "usearch_b200_export_keys", "usearch_b200_export_keys_at", "usearch_b200_copy",
+    "usearch_b200_levels_stats", "usearch_b200_multi",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -188,6 +190,18 @@ def load_library() -> C.CDLL:
     lib.usearch_b200_indexes_last_ms.argtypes = [C.c_void_p, C.c_void_p]
     lib.usearch_b200_merge_into.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p,
                                             C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_get_many.restype = C.c_size_t
+    lib.usearch_b200_get_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p,
+                                          err]
+    lib.usearch_b200_export_keys.restype = C.c_size_t
+    lib.usearch_b200_export_keys.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, err]
+    lib.usearch_b200_export_keys_at.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, err]
+    lib.usearch_b200_copy.restype = C.c_void_p
+    lib.usearch_b200_copy.argtypes = [C.c_void_p, err]
+    lib.usearch_b200_levels_stats.restype = C.c_size_t
+    lib.usearch_b200_levels_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, err]
+    lib.usearch_b200_multi.restype = C.c_bool
+    lib.usearch_b200_multi.argtypes = [C.c_void_p]
     lib.usearch_distance.restype = C.c_float
     lib.usearch_distance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_size_t, C.c_int, err]
     _lib = lib
@@ -197,6 +211,90 @@ def load_library() -> C.CDLL:
 def _raise(err: C.c_char_p) -> None:
     if err.value:
         raise RuntimeError(err.value.decode())
+
+
+_KIND_TO_NP = {"f32": np.float32, "f64": np.float64, "f16": np.float16, "bf16": np.uint16, "i8": np.int8, "b1": np.uint8}
+_NODE_HEAD_BYTES = 10  # a node's key and level in the reference's tape (index.hpp:2116-2195)
+
+
+def _normalize_kind(dtype) -> str:
+    """A kind name, or a NumPy dtype as the reference's `_normalize_dtype` maps it (uint8 -> b1); bf16 by name only."""
+    if isinstance(dtype, str) and dtype in SCALAR_KIND:
+        return dtype
+    try:
+        kind = _NP_TO_SCALAR.get(np.dtype(dtype))
+    except TypeError:
+        kind = None
+    if kind is None:
+        raise ValueError(f"Unsupported dtype {dtype!r}")
+    return kind
+
+
+def _as_keys(keys) -> np.ndarray:
+    """Any iterable or integer array of keys, any stride -> a dense uint64 array."""
+    if not isinstance(keys, np.ndarray):
+        keys = np.fromiter((int(k) for k in keys), dtype=np.uint64)
+    if keys.ndim != 1:
+        raise ValueError("Keys must be placed in a single-dimensional array")
+    return np.ascontiguousarray(keys, dtype=np.uint64)
+
+
+@dataclass(frozen=True)
+class IndexStats:
+    """`index_gt::stats_t` (index.hpp:3133-3138)."""
+    nodes: int
+    edges: int
+    max_edges: int
+    allocated_bytes: int
+
+
+class IndexedKeys:
+    """The live keys of an index in slot order (index.py:453-488): `len`, `[i]` (negative too), slices, integer arrays of
+    offsets, `__array__` and iteration. Each call reads the keys once on the host."""
+
+    def __init__(self, index: "Index") -> None:
+        self.index = index
+
+    def __len__(self) -> int:
+        return len(self.index)
+
+    def _slice(self, offset: int, limit: int) -> np.ndarray:
+        out = np.zeros(max(limit, 0), dtype=np.uint64)
+        err = C.c_char_p()
+        n = self.index._lib.usearch_b200_export_keys(self.index._h, offset, out.size, out.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        return out[:n]
+
+    def _at(self, offsets) -> np.ndarray:
+        offsets = np.asarray(offsets, dtype=np.int64).ravel()
+        size = len(self)
+        offsets = np.where(offsets < 0, offsets + size, offsets)
+        if offsets.size and (offsets.min() < 0 or offsets.max() >= size):
+            raise IndexError("Index out of range")
+        offsets = np.ascontiguousarray(offsets, dtype=np.uintp)
+        out = np.zeros(offsets.size, dtype=np.uint64)
+        err = C.c_char_p()
+        self.index._lib.usearch_b200_export_keys_at(self.index._h, offsets.ctypes.data_as(C.c_void_p), offsets.size,
+                                                    out.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        return out
+
+    def __getitem__(self, at):
+        if isinstance(at, slice):
+            start, stop, step = at.indices(len(self))
+            if step == 1:
+                return self._slice(start, stop - start)
+            return self._at(np.arange(start, stop, step))
+        if np.isscalar(at) or isinstance(at, int):
+            return int(self._at([int(at)])[0])
+        return self._at(at)
+
+    def __array__(self, dtype=None, copy=None):
+        keys = self._slice(0, len(self))
+        return keys if dtype is None else keys.astype(dtype)
+
+    def __iter__(self):
+        return iter(self._slice(0, len(self)).tolist())
 
 
 @dataclass
@@ -421,18 +519,116 @@ class Index:
             return int(self._lib.usearch_count(self._h, int(keys), None))
         return self._count_many(keys).astype(np.uint64)
 
-    def get(self, key: int, dtype: Optional[str] = None, count: int = 1) -> Optional[np.ndarray]:
-        """`Index.get` (index.py:820-870): the vector(s) stored under `key`, or None."""
-        kind = dtype or self._dtype
-        np_t = {"f32": np.float32, "f64": np.float64, "f16": np.float16, "bf16": np.uint16, "i8": np.int8, "b1": np.uint8}[kind]
+    def get(self, keys, dtype=None, count: int = 1):
+        """`Index.get` (index.py:765-809). One key: the vector stored under it (`count` > 1: up to that many rows), or
+        None. An iterable or array of keys: on a plain index an ``[n, ndim]`` array, a missing key's row zero; on a multi
+        index a tuple holding, per key, the matrix of all its vectors in insertion order, or None. `dtype` is one of the
+        kind names, or a NumPy dtype as the reference maps it (uint8 means b1); bf16 comes back as uint16 words."""
+        kind = _normalize_kind(dtype) if dtype is not None else self._dtype
+        np_t = _KIND_TO_NP[kind]
         cols = (self.ndim + 7) // 8 if kind == "b1" else self.ndim
-        out = np.zeros((count, cols), dtype=np_t)
+        if np.isscalar(keys) or isinstance(keys, int) or (isinstance(keys, np.ndarray) and keys.ndim == 0):
+            out = np.zeros((count, cols), dtype=np_t)
+            err = C.c_char_p()
+            found = self._lib.usearch_get(self._h, int(keys), count, out.ctypes.data_as(C.c_void_p), SCALAR_KIND[kind],
+                                          C.byref(err))
+            _raise(err)
+            if not found:
+                return None
+            return out[0] if count == 1 else out[:found]
+        keys = _as_keys(keys)
+        n = keys.shape[0]
+        multi = self.multi
+        if multi:
+            rows = int(self._count_many(keys).sum())
+            per_key = np.iinfo(np.uint64).max
+        else:
+            rows, per_key = n, 1
+        out = np.zeros((rows, cols), dtype=np_t)
+        counts = np.zeros(n, dtype=np.uintp)
         err = C.c_char_p()
-        found = self._lib.usearch_get(self._h, int(key), count, out.ctypes.data_as(C.c_void_p), SCALAR_KIND[kind], C.byref(err))
+        got = self._lib.usearch_b200_get_many(self._h, keys.ctypes.data_as(C.c_void_p), n, C.c_size_t(per_key),
+                                              out.ctypes.data_as(C.c_void_p), out.strides[0] if rows else 0, SCALAR_KIND[kind],
+                                              counts.ctypes.data_as(C.c_void_p), C.byref(err))
         _raise(err)
-        if not found:
-            return None
-        return out[0] if count == 1 else out[:found]
+        if multi:
+            ends = np.cumsum(counts.astype(np.int64))
+            return tuple(out[e - int(c):e] if c else None for c, e in zip(counts, ends))
+        if got == n:
+            return out
+        full = np.zeros((n, cols), dtype=np_t)
+        full[counts.astype(bool)] = out[:got]
+        return full
+
+    def __getitem__(self, keys):
+        return self.get(keys)
+
+    def __delitem__(self, keys) -> None:
+        self.remove(keys)
+
+    @property
+    def keys(self) -> "IndexedKeys":
+        """Every live key, in slot order (the reference lists them in its hash table's order)."""
+        return IndexedKeys(self)
+
+    @property
+    def vectors(self):
+        """`get(keys)` for every live key, in the order of `keys`."""
+        return self.get(np.asarray(self.keys))
+
+    @property
+    def multi(self) -> bool:
+        return bool(self._lib.usearch_b200_multi(self._h))
+
+    @property
+    def nlevels(self) -> int:
+        return self.max_level + 1
+
+    def copy(self) -> "Index":
+        """`Index.copy` (index.py:1152-1168): an independent index on the same GPU with the same contents, configuration,
+        removed-slot queue and knobs. It stays valid when this one is deleted."""
+        err = C.c_char_p()
+        handle = self._lib.usearch_b200_copy(self._h, C.byref(err))
+        _raise(err)
+        result = Index.__new__(Index)
+        result.__dict__.update(self.__dict__)
+        result._h = C.c_void_p(handle)
+        result._keepalive = None
+        result.last_join_stats, result.last_join_ms = {}, {}
+        return result
+
+    def reset(self) -> None:
+        """Release the index's device memory and keep its configuration: a later `add` starts a new graph."""
+        self._lib.usearch_clear(self._h, None)
+
+    def _levels_stats(self):
+        err = C.c_char_p()
+        total = np.zeros(4, dtype=np.uintp)
+        levels = self._lib.usearch_b200_levels_stats(self._h, None, 0, total.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        per = np.zeros((max(levels, 1), 4), dtype=np.uintp)
+        levels = self._lib.usearch_b200_levels_stats(self._h, per.ctypes.data_as(C.c_void_p), levels, None, C.byref(err))
+        _raise(err)
+        return [IndexStats(*(int(v) for v in row)) for row in per[:levels]], IndexStats(*(int(v) for v in total))
+
+    @property
+    def stats(self) -> "IndexStats":
+        """`index_gt::stats()` over every node: nodes, edges, max_edges and allocated_bytes (the reference's node layout,
+        not HBM use: see `memory_usage`)."""
+        return self._levels_stats()[1]
+
+    @property
+    def levels_stats(self) -> list:
+        """`index_gt::stats(stats_per_level, max_level)`: one entry per level, the node head counted on level 0 only."""
+        return self._levels_stats()[0]
+
+    def level_stats(self, level: int) -> "IndexStats":
+        """`index_gt::stats(level)`: the nodes on `level` and above, the node head counted on every level."""
+        per = self._levels_stats()[0]
+        if level >= len(per):
+            return IndexStats(0, 0, 0, 0)
+        s = per[level]
+        return s if level == 0 else IndexStats(s.nodes, s.edges, s.max_edges, s.allocated_bytes + _NODE_HEAD_BYTES * s.nodes)
 
     def remove(self, keys, *, compact: bool = False, threads: int = 0) -> int:
         """`Index.remove` (python/lib.cpp:1192-1227): one key or an iterable of keys; returns the number of entries
