@@ -310,6 +310,32 @@ void usearch_b200_search_many_device(usearch_index_t index, void const* queries,
                                      usearch_distance_t* distances, uint32_t* counts, uint32_t* computed_distances,
                                      uint32_t* visited_members, void* cuda_stream, usearch_error_t* error);
 
+/* Lookups by key from DEVICE memory, for keys that a device pipeline produced (e.g. the keys of
+ * usearch_b200_search_many_device). They follow usearch_b200_search_many_device: all pointers are DEVICE pointers on the
+ * index's GPU, the work runs on `cuda_stream` (NULL = the handle's own stream) and the call returns when the outputs are
+ * complete. count and get probe a key -> slot table in HBM (16 bytes per cell, at least twice as many cells as live
+ * entries), built on the first such lookup after the keys changed and counted by usearch_memory_usage from then on. */
+
+/* counts[i] = entries stored under keys[i] (usearch_b200_count_many). */
+void usearch_b200_count_many_device(usearch_index_t index, usearch_key_t const* keys, size_t count, uint32_t* counts,
+                                    void* cuda_stream, usearch_error_t* error);
+/* usearch_b200_get_many with DEVICE keys and outputs. Key i owns rows i*max_per_key .. i*max_per_key+max_per_key-1 of
+ * `vectors` (`vectors_stride` bytes apart, 0 = packed), cast to `kind`; counts[i] = the rows written for key i, and rows
+ * past counts[i] are zero. A key's rows are its min(count, max_per_key) lowest slots (its oldest entries) in ascending
+ * order: what usearch_b200_get_many returns whenever max_per_key >= the key's count, or the index holds no removed
+ * entries. */
+void usearch_b200_get_many_device(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t max_per_key,
+                                  void* vectors, size_t vectors_stride, usearch_scalar_kind_t kind, uint32_t* counts,
+                                  void* cuda_stream, usearch_error_t* error);
+/* usearch_b200_filtered_search_many with DEVICE queries (in the index's kind), DEVICE allowed keys and DEVICE outputs,
+ * laid out as in usearch_b200_search_many_device. The allowed keys are sorted on the device; the result equals the host
+ * call's with the same keys. */
+void usearch_b200_filtered_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                              size_t queries_stride, size_t count, usearch_key_t const* allowed_keys,
+                                              size_t allowed_count, usearch_key_t* keys, usearch_distance_t* distances,
+                                              uint32_t* counts, uint32_t* computed_distances, uint32_t* visited_members,
+                                              void* cuda_stream, usearch_error_t* error);
+
 /* The asynchronous pair. `enqueue` = the same arguments as usearch_b200_search_many_device, but it ONLY enqueues the
  * kernel on `cuda_stream` and returns; any number of batches may be in flight. `finish` waits for them, inspects the
  * per-query status words and re-runs, with larger scratch, the rare queries whose scratch overflowed; the outputs of

@@ -273,6 +273,31 @@ class index_dense_t {
         return usearch_b200_get_many(handle_, keys, count, vectors_per_key, vectors, 0, scalar_kind<scalar_at>(),
                                      counts ? counts : own.data(), &error);
     }
+    /* lookups by key from DEVICE memory (usearch_b200_count_many_device, _get_many_device, _filtered_search_many_device):
+     * every pointer is a device pointer on the index's GPU, `cuda_stream` a cudaStream_t (NULL = the handle's stream) */
+    error_t count_device(vector_key_t const* keys, std::size_t count, std::uint32_t* counts, void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_count_many_device(handle_, keys, count, counts, cuda_stream, &e);
+        return e;
+    }
+    /* key i owns rows i * vectors_per_key .. of `vectors`, its oldest entries first; rows past counts[i] are zero */
+    template <typename scalar_at>
+    error_t get_device(vector_key_t const* keys, std::size_t count, scalar_at* vectors, std::uint32_t* counts,
+                       std::size_t vectors_per_key = 1, std::size_t stride_bytes = 0, void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_get_many_device(handle_, keys, count, vectors_per_key, vectors, stride_bytes, scalar_kind<scalar_at>(), counts,
+                                     cuda_stream, &e);
+        return e;
+    }
+    error_t filtered_search_device(void const* queries, std::size_t queries_count, std::size_t queries_stride, std::size_t wanted,
+                                   vector_key_t const* allowed_keys, std::size_t allowed_count, vector_key_t* keys,
+                                   distance_t* distances, std::uint32_t* counts, std::uint32_t* computed_distances = nullptr,
+                                   std::uint32_t* visited_members = nullptr, void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_filtered_search_many_device(handle_, queries, queries_count, queries_stride, wanted, allowed_keys, allowed_count,
+                                                 keys, distances, counts, computed_distances, visited_members, cuda_stream, &e);
+        return e;
+    }
     /* index_dense.hpp:1595-1608, the live keys in slot order */
     void export_keys(vector_key_t* keys, std::size_t offset, std::size_t limit) const {
         usearch_b200_export_keys(handle_, offset, limit, keys, nullptr);

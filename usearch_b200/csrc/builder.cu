@@ -830,6 +830,7 @@ char const* frozen_index_t::add_many(uint64_t const* new_keys, void const* vecto
                                      bool on_device) {
     if (!count) return nullptr;
     if (char const* e = ensure_context()) return e;
+    keys_generation += 1;
     if (!configured()) return "Index is not initialized: call usearch_init with options or load a file first";
     if (!bits_per_scalar(kind)) return "Unknown scalar kind!";
     size_t const reused = reuse_removed ? std::min(count, free_slots.size()) : 0;
@@ -1135,6 +1136,7 @@ char const* frozen_index_t::remove_many(uint64_t const* keys, size_t count, bool
     if (pruned) *pruned = 0;
     if (!loaded || !size) return nullptr;
     if (char const* e = ensure_context()) return e;
+    keys_generation += 1;
     build_key_map();
     std::vector<uint32_t> slots;
     for (size_t i = 0; i < count; ++i) {

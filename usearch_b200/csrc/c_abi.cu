@@ -179,7 +179,9 @@ usearch_index_t usearch_init(usearch_init_options_t* options, usearch_error_t* e
 
 void usearch_free(usearch_index_t index, usearch_error_t*) { delete as_index(index); }
 
-size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { return as_index(index)->hbm_bytes; }
+size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table counts once it exists */
+    return as_index(index)->hbm_bytes + as_index(index)->key_table.cells.capacity * sizeof(key_cell_t);
+}
 
 char const* usearch_hardware_acceleration(usearch_index_t, usearch_error_t*) { return "sm_90a"; }
 
@@ -363,6 +365,46 @@ void usearch_b200_search_many_device(usearch_index_t index, void const* queries,
     cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream;
     set_error(error, ix->search_device(queries, queries_count, queries_stride, count, keys, distances, counts,
                                        computed_distances, visited_members, s));
+}
+
+/* lookups by key from device memory (device_keys.cu), on the caller's stream like usearch_b200_search_many_device */
+void usearch_b200_count_many_device(usearch_index_t index, usearch_key_t const* keys, size_t count, uint32_t* counts,
+                                    void* cuda_stream, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        return ix->count_many_device(keys, count, counts, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
+    }));
+}
+
+void usearch_b200_get_many_device(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t max_per_key,
+                                  void* vectors, size_t vectors_stride, usearch_scalar_kind_t kind, uint32_t* counts,
+                                  void* cuda_stream, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        uint32_t const vs = scalar_to_char(kind);
+        if (!vs) return "Unknown scalar kind!";
+        return ix->get_many_device(keys, count, max_per_key, vectors, vectors_stride, vs, counts,
+                                   cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
+    }));
+}
+
+void usearch_b200_filtered_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                              size_t queries_stride, size_t count, usearch_key_t const* allowed_keys,
+                                              size_t allowed_count, usearch_key_t* keys, usearch_distance_t* distances,
+                                              uint32_t* counts, uint32_t* computed_distances, uint32_t* visited_members,
+                                              void* cuda_stream, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        return ix->filtered_search_device(queries, queries_count, queries_stride, count, allowed_keys, allowed_count, keys, distances,
+                                          counts, computed_distances, visited_members,
+                                          cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
+    }));
 }
 
 /* the asynchronous pair: enqueue any number of batches (kernel launches only, nothing waits), then finish once */

@@ -65,6 +65,8 @@ void frozen_index_t::release_device() {
     levels.clear();
     host_keys.clear();
     key_map.clear();
+    key_table = key_table_t{};
+    keys_generation += 1;
 }
 
 char const* frozen_index_t::ensure_context() {
@@ -950,6 +952,7 @@ char const* pair_distance_host(void const* a, void const* b, uint32_t scalar, si
 char const* frozen_index_t::rename_key(uint64_t from, uint64_t to, size_t* renamed) {
     *renamed = 0;
     if (!loaded || !size) return nullptr;
+    keys_generation += 1;
     if (char const* e = ensure_context()) return e;
     if (to == free_key) return "Key is reserved for removed entries";
     build_key_map();

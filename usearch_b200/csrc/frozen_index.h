@@ -17,6 +17,7 @@
 
 #include "cuda_buffers.h"
 #include "device_index.h"
+#include "device_keys.h"
 #include "key_map.h"
 
 namespace usearch_b200 {
@@ -98,6 +99,9 @@ struct frozen_index_t {
     uint64_t level_seed = 0;
     bool configured() const { return metric && scalar && dimensions && connectivity; }
     void build_key_map() { if (!key_map.built) key_map.rebuild(host_keys, free_key, capacity); }
+    /* bumped by every call that can change the key -> slot relation (add, remove, rename, clear, load): a device key
+     * table built at another generation is stale */
+    uint64_t keys_generation = 0;
 
     /* device */
     cuda_stream_t stream; /* the handle's device (`stream.device`), its SM count and the handle's own stream */
@@ -204,6 +208,21 @@ struct frozen_index_t {
                                       uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles, cudaStream_t stream);
     char const* sharded_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t* keys,
                                     float* dists, size_t* counts);
+
+    /* device_keys.cu: lookups by key from device memory, through a key -> slot table in HBM built on first use */
+    struct key_table_t {
+        device_buffer_t<key_cell_t> cells;
+        uint64_t mask = 0, generation = 0;
+    } key_table;
+    device_buffer_t<uint32_t> lookup_slots; /* get_many_device: the slot of every output row */
+    device_buffer_t<uint8_t> lookup_gathered, lookup_casted, allowed_sort_temp;
+    char const* ensure_key_table(cudaStream_t s);
+    char const* count_many_device(uint64_t const* keys, size_t n, uint32_t* counts, cudaStream_t s);
+    char const* get_many_device(uint64_t const* keys, size_t n, size_t max_per_key, void* out, size_t out_stride, uint32_t out_scalar,
+                                uint32_t* counts, cudaStream_t s);
+    char const* filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t const* allowed,
+                                       size_t allowed_count, uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed,
+                                       uint32_t* d_visited, cudaStream_t s);
 
     /* searches */
     char const* plan(uint32_t k, uint32_t visited_cap_override, launch_plan_t& plan, uint32_t ef_override = 0) const;

@@ -10,7 +10,19 @@
 
 #include "device_index.h"
 
+#ifdef __CUDACC__
+#define USEARCH_B200_HOST_DEVICE __host__ __device__
+#else
+#define USEARCH_B200_HOST_DEVICE
+#endif
+
 namespace usearch_b200 {
+
+/* the 64-bit finalizer both key tables hash with: key_map_t here and the table in HBM (device_keys.h) */
+USEARCH_B200_HOST_DEVICE inline uint64_t key_hash(uint64_t k) {
+    k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+    return k;
+}
 
 /* key -> slot(s): open addressing over the host copy of the keys, built on first use. Plays the role of
  * index_dense_gt::slot_lookup_ (index_dense.hpp:462-500); a `multi` index keeps one entry per (key, slot). */
@@ -20,10 +32,7 @@ struct key_map_t {
     size_t used = 0;
     bool built = false;
     static constexpr uint32_t TOMB = 0xFFFFFFFEu;
-    static size_t hash(uint64_t k) {
-        k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-        return (size_t)k;
-    }
+    static size_t hash(uint64_t k) { return (size_t)key_hash(k); }
     void clear() { cells.clear(); used = 0; built = false; }
     void rebuild(std::vector<uint64_t> const& host_keys, uint64_t free_key, size_t expect) {
         keys = &host_keys;

@@ -59,7 +59,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_last_join_ms", "usearch_b200_indexes_init", "usearch_b200_indexes_free", "usearch_b200_indexes_merge",
     "usearch_b200_indexes_size", "usearch_b200_indexes_search_many", "usearch_b200_indexes_last_ms", "usearch_b200_merge_into",
     "usearch_b200_get_many", "usearch_b200_export_keys", "usearch_b200_export_keys_at", "usearch_b200_copy",
-    "usearch_b200_levels_stats", "usearch_b200_multi",
+    "usearch_b200_levels_stats", "usearch_b200_multi", "usearch_b200_count_many_device", "usearch_b200_get_many_device",
+    "usearch_b200_filtered_search_many_device",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -111,6 +112,12 @@ def load_library() -> C.CDLL:
                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                     C.c_void_p, err]
     lib.usearch_b200_search_many_enqueue.argtypes = lib.usearch_b200_search_many_device.argtypes
+    lib.usearch_b200_count_many_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_get_many_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                 C.c_int, C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_filtered_search_many_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                             C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                             C.c_void_p, C.c_void_p, C.c_void_p, err]
     lib.usearch_b200_search_many_finish.argtypes = [C.c_void_p, err]
     lib.usearch_b200_tune.restype = C.c_int
     lib.usearch_b200_tune.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
@@ -916,6 +923,36 @@ class Index:
         self._lib.usearch_b200_search_many_device(self._h, queries_ptr, nq, stride, count, keys_ptr, distances_ptr,
                                                   counts_ptr, computed_ptr or None, visited_ptr or None,
                                                   stream or None, C.byref(err))
+        _raise(err)
+
+    def count_device(self, keys_ptr: int, n: int, counts_ptr: int, stream: int = 0) -> None:
+        """`count` for `n` keys in DEVICE memory: counts (uint32 [n], device) = the entries stored under each key.
+        `contains` is ``counts > 0``."""
+        err = C.c_char_p()
+        self._lib.usearch_b200_count_many_device(self._h, keys_ptr, n, counts_ptr, stream or None, C.byref(err))
+        _raise(err)
+
+    def get_device(self, keys_ptr: int, n: int, vectors_ptr: int, counts_ptr: int, count: int = 1, stride: int = 0,
+                   dtype: Optional[str] = None, stream: int = 0) -> None:
+        """`get` for `n` keys in DEVICE memory into DEVICE rows: key i owns rows ``i * count`` .. ``i * count + count - 1``
+        of `vectors` (`stride` bytes apart, 0 = packed) in `dtype` (default: the index's kind); counts (uint32 [n]) get
+        the rows written per key, and the rows past them are zero. A key's rows are its `count` oldest entries."""
+        kind = _normalize_kind(dtype) if dtype is not None else self._dtype
+        err = C.c_char_p()
+        self._lib.usearch_b200_get_many_device(self._h, keys_ptr, n, C.c_size_t(count), vectors_ptr, stride, SCALAR_KIND[kind],
+                                               counts_ptr, stream or None, C.byref(err))
+        _raise(err)
+
+    def filtered_search_device(self, queries_ptr: int, nq: int, stride: int, count: int, allowed_ptr: int, allowed_count: int,
+                               keys_ptr: int, distances_ptr: int, counts_ptr: int, computed_ptr: int = 0, visited_ptr: int = 0,
+                               stream: int = 0) -> None:
+        """`search_device` restricted to `allowed_count` keys held in DEVICE memory (uint64): the result of
+        `filtered_search` with the same keys."""
+        err = C.c_char_p()
+        self._lib.usearch_b200_filtered_search_many_device(self._h, queries_ptr, nq, stride, count, allowed_ptr or None,
+                                                           allowed_count, keys_ptr, distances_ptr, counts_ptr,
+                                                           computed_ptr or None, visited_ptr or None, stream or None,
+                                                           C.byref(err))
         _raise(err)
 
 
