@@ -25,7 +25,9 @@
  *  QT x VT accumulator sets in registers: one stage read feeds QT pairs and one (broadcast) query read feeds VT x 8
  *  groups. The k-best lists live in global memory (L2): after the first few tiles an insertion is a rare event.
  *
- *  exact_scan_kernel (fallback when the tiled stage does not fit in 227 KB): one query per warp, list in registers.
+ *  exact_scan_kernel (fallback when the tiled stage does not fit in 227 KB): one query per warp, list in registers. Its
+ *  own stage (8 queries and 2 x 32/LPV rows) holds f32 rows up to 2400 dims; longer rows are read in place from global
+ *  memory by the same kernel (STAGED = false), so exact search serves any length the index does.
  */
 #include <cuda_runtime.h>
 
@@ -62,31 +64,45 @@ __device__ __forceinline__ float finish_ordered(typename M::acc_t const& acc, ty
     else return M::finish(acc, qc);
 }
 
-template <class M, bool SWAP>
+/* a 16-byte chunk of a staged row (shared memory) or of a row read in place (global memory, read-only path) */
+template <bool STAGED> __device__ __forceinline__ uint4 scan_chunk(uint4 const* p) {
+    if constexpr (STAGED) return *p;
+    else return __ldg(p);
+}
+
+/* STAGED = false: the query and the rows are read from global memory where they lie, for rows too long to stage 8 queries
+ * and 2 x VPP rows in 227 KB. Each lane group walks the same chunks in the same order through the same metric calls,
+ * so both variants give the same bits. */
+template <class M, bool SWAP, bool STAGED>
 __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_constant__ device_index_t const ix,
                                                                       __grid_constant__ exact_args_t const a) {
     constexpr int LPV = M::LPV, VPP = 32 / LPV;
     extern __shared__ __align__(128) uint8_t smem[];
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane / LPV, sub = lane % LPV;
     uint32_t const chunks = ix.chunks16, bytes = (uint32_t)ix.vec_stride;
-    uint4* const q4 = reinterpret_cast<uint4*>(smem + (size_t)warp * bytes);
     uint32_t const bars = smem_u32(smem + a.off_bars), stage_addr = smem_u32(smem + a.off_stage);
     uint32_t const qi = blockIdx.x * EXACT_WARPS + warp;
     bool const has_query = qi < a.nq;
     uint32_t const seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
     uint32_t const ntiles = seg_hi > seg_lo ? (seg_hi - seg_lo + VPP - 1) / VPP : 0;
-
-    if (threadIdx.x == 0) {
-        mbar_init(bars, 1);
-        mbar_init(bars + 8, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    uint4 const* q4; /* a dead query slot reads query 0: prepare() shuffles across the whole warp */
+    if constexpr (STAGED) {
+        uint4* const q4s = reinterpret_cast<uint4*>(smem + (size_t)warp * bytes);
+        q4 = q4s;
+        if (threadIdx.x == 0) {
+            mbar_init(bars, 1);
+            mbar_init(bars + 8, 1);
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        }
+        if (has_query) {
+            uint4 const* src = reinterpret_cast<uint4 const*>(a.queries + (size_t)qi * a.query_stride);
+            for (uint32_t j = lane; j < chunks; j += 32) q4s[j] = src[j];
+        }
+        __syncthreads();
+    } else {
+        q4 = reinterpret_cast<uint4 const*>(a.queries + (size_t)(has_query ? qi : 0u) * a.query_stride);
     }
-    if (has_query) {
-        uint4 const* src = reinterpret_cast<uint4 const*>(a.queries + (size_t)qi * a.query_stride);
-        for (uint32_t j = lane; j < chunks; j += 32) q4[j] = src[j];
-    }
-    __syncthreads();
     typename M::qconst_t qc = M::prepare(q4, chunks, lane);
     typename rnorm_of<M>::type q_rn = 0;
     if constexpr (M::NORMS) q_rn = rnorm_of<M>::get(qc.a2);
@@ -98,7 +114,8 @@ __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_con
             bulk_copy_g2s(stage_addr + (set * VPP + i) * a.stage_stride, ix.vectors + (size_t)(base + i) * ix.vec_stride, bytes,
                           bars + 8u * set);
     };
-    if (threadIdx.x == 0 && ntiles) issue(0);
+    if constexpr (STAGED)
+        if (threadIdx.x == 0 && ntiles) issue(0);
 
     float td[TOP_E];
     uint32_t ts[TOP_E];
@@ -109,25 +126,30 @@ __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_con
 
     for (uint32_t t = 0; t < ntiles; ++t) {
         uint32_t const set = t & 1u, base = seg_lo + t * VPP, cnt = min((uint32_t)VPP, seg_hi - base);
-        if (threadIdx.x == 0 && t + 1 < ntiles) issue(t + 1); /* the other set was released by the barrier below */
-        mbar_wait(bars + 8u * set, (phase >> set) & 1u);
-        phase ^= 1u << set;
+        if constexpr (STAGED) {
+            if (threadIdx.x == 0 && t + 1 < ntiles) issue(t + 1); /* the other set was released by the barrier below */
+            mbar_wait(bars + 8u * set, (phase >> set) & 1u);
+            phase ^= 1u << set;
+        }
         uint32_t const slot = base + (uint32_t)g;
         bool const act = has_query && (uint32_t)g < cnt;
         typename M::acc_t acc;
         M::init(acc);
         if (act) {
-            uint4 const* buf = reinterpret_cast<uint4 const*>(smem + a.off_stage + (size_t)(set * VPP + g) * a.stage_stride);
+            uint4 const* buf = STAGED ? reinterpret_cast<uint4 const*>(smem + a.off_stage + (size_t)(set * VPP + g) * a.stage_stride)
+                                      : reinterpret_cast<uint4 const*>(ix.vectors + (size_t)slot * ix.vec_stride);
             uint32_t j = sub;
             for (; j + 3 * LPV < chunks; j += 4 * LPV) {
-                uint4 b0 = buf[j], b1 = buf[j + LPV], b2 = buf[j + 2 * LPV], b3 = buf[j + 3 * LPV];
-                uint4 q0 = q4[j], q1 = q4[j + LPV], q2 = q4[j + 2 * LPV], q3 = q4[j + 3 * LPV];
+                uint4 b0 = scan_chunk<STAGED>(buf + j), b1 = scan_chunk<STAGED>(buf + j + LPV), b2 = scan_chunk<STAGED>(buf + j + 2 * LPV),
+                      b3 = scan_chunk<STAGED>(buf + j + 3 * LPV);
+                uint4 q0 = scan_chunk<STAGED>(q4 + j), q1 = scan_chunk<STAGED>(q4 + j + LPV), q2 = scan_chunk<STAGED>(q4 + j + 2 * LPV),
+                      q3 = scan_chunk<STAGED>(q4 + j + 3 * LPV);
                 M::step(acc, b0, q0);
                 M::step(acc, b1, q1);
                 M::step(acc, b2, q2);
                 M::step(acc, b3, q3);
             }
-            for (; j < chunks; j += LPV) M::step(acc, buf[j], q4[j]);
+            for (; j < chunks; j += LPV) M::step(acc, scan_chunk<STAGED>(buf + j), scan_chunk<STAGED>(q4 + j));
         }
         float d = finish_ordered<M, SWAP>(acc, qc);
         if constexpr (M::NORMS) {
@@ -150,7 +172,7 @@ __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_con
                 worst = top_back_reg(td, top_size);
             }
         }
-        __syncthreads(); /* every warp is done with this set before thread 0 refills it */
+        if constexpr (STAGED) __syncthreads(); /* every warp is done with this set before thread 0 refills it */
     }
 
     if (has_query) { /* partial result of this (query, segment) */
@@ -365,18 +387,24 @@ __global__ void exact_merge_big_kernel(device_index_t ix, exact_args_t a, float*
     if (lane == 0) a.out_counts[qi] = top_size;
 }
 
-template <class M> static cudaError_t exact_launch_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, size_t smem,
-                                                     cudaStream_t stream) {
+template <class M, bool STAGED> static cudaError_t exact_launch_scan_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid,
+                                                                      size_t smem, cudaStream_t stream) {
     if (swap) {
-        cudaError_t e = cudaFuncSetAttribute(exact_scan_kernel<M, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(exact_scan_kernel<M, true, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        exact_scan_kernel<M, true><<<grid, EXACT_WARPS * 32, smem, stream>>>(ix, a);
+        exact_scan_kernel<M, true, STAGED><<<grid, EXACT_WARPS * 32, smem, stream>>>(ix, a);
     } else {
-        cudaError_t e = cudaFuncSetAttribute(exact_scan_kernel<M, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(exact_scan_kernel<M, false, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        exact_scan_kernel<M, false><<<grid, EXACT_WARPS * 32, smem, stream>>>(ix, a);
+        exact_scan_kernel<M, false, STAGED><<<grid, EXACT_WARPS * 32, smem, stream>>>(ix, a);
     }
     return cudaGetLastError();
+}
+
+/* smem == 0: the staged scan does not fit, rows are read in place */
+template <class M> static cudaError_t exact_launch_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, size_t smem,
+                                                     cudaStream_t stream) {
+    return smem ? exact_launch_scan_t<M, true>(ix, a, swap, grid, smem, stream) : exact_launch_scan_t<M, false>(ix, a, swap, grid, 0, stream);
 }
 
 template <class M> static cudaError_t exact_launch_tiled_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, size_t smem,
@@ -454,11 +482,14 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     a.off_bars = off;
     off = (off + 16 + 127) / 128 * 128;
     a.off_stage = off;
-    size_t const smem = wgmma ? exact_wgmma_smem_bytes() : (imma ? exact_imma_smem_bytes() : off + 2 * (size_t)vpp * a.stage_stride);
-    if (smem > 227 * 1024) return "Vectors too long for the exact-search stage";
+    size_t smem = wgmma ? exact_wgmma_smem_bytes() : (imma ? exact_imma_smem_bytes() : off + 2 * (size_t)vpp * a.stage_stride);
+    /* only the one-query-per-warp scan can outgrow its stage (the tiled one is not chosen then): it reads in place */
+    bool const in_place = smem > 227 * 1024;
+    if (in_place) smem = 0;
     uint32_t const groups = (uint32_t)((nq + qpc - 1) / qpc);
-    /* cut the dataset so that the grid fills whole waves of the resident CTAs (1 per SM tiled, ~3 per SM otherwise) */
-    uint32_t const resident = (uint32_t)sm_count * (wgmma ? 1u : (imma ? 2u : (tiled ? 1u : 3u)));
+    /* cut the dataset so that the grid fills whole waves of the resident CTAs (1 per SM tiled, ~3 per SM staged, 4 per SM
+     * in place: up to 64 registers) */
+    uint32_t const resident = (uint32_t)sm_count * (wgmma ? 1u : (imma ? 2u : (tiled ? 1u : (in_place ? 4u : 3u))));
     uint32_t const max_segments = std::max<uint32_t>(1, std::min<uint32_t>((ix.n + 8 * (uint32_t)vpp - 1) / (8 * (uint32_t)vpp), 65535u));
     uint32_t segments = 1;
     {
