@@ -336,6 +336,30 @@ void usearch_b200_filtered_search_many_device(usearch_index_t index, void const*
                                               uint32_t* counts, uint32_t* computed_distances, uint32_t* visited_members,
                                               void* cuda_stream, usearch_error_t* error);
 
+/* Grouped filtered search: one batch in which every query has its own allowed key set. The sets are given as CSR:
+ * set g holds set_keys[offsets[g] .. offsets[g + 1]] (`sets_count` + 1 offsets, the first 0, never decreasing; a set may
+ * be empty, repeat keys or name keys the index lacks), and query i uses set groups[i] < sets_count. Row i equals
+ * usearch_b200_filtered_search_many(queries[i], count, that set): keys, distances, counts and both counters. Every set
+ * becomes a bitmap row over slots; the rows of as many sets as the "group_bitmap_mb" knob allows (default 1024 MB) are
+ * served per launch. A group id out of range, bad offsets or no sets for a non-empty batch are refused before any output
+ * is written; so is a sharded handle. Buffers are HOST memory; queries may be of any kind (cast on the device). Returns
+ * the sum of counts. */
+size_t usearch_b200_grouped_filtered_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                 size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                 uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                 usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                 size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
+                                                 usearch_error_t* error);
+/* The same with DEVICE queries (in the index's kind), DEVICE groups, offsets, set keys and outputs, laid out as in
+ * usearch_b200_search_many_device, on `cuda_stream` (NULL = the handle's stream). The arguments are checked on the device
+ * before the search; the call returns when the outputs are complete. */
+void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                      size_t queries_stride, size_t count, uint32_t const* groups,
+                                                      uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                      usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                      uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
+                                                      usearch_error_t* error);
+
 /* The asynchronous pair. `enqueue` = the same arguments as usearch_b200_search_many_device, but it ONLY enqueues the
  * kernel on `cuda_stream` and returns; any number of batches may be in flight. `finish` waits for them, inspects the
  * per-query status words and re-runs, with larger scratch, the rare queries whose scratch overflowed; the outputs of
@@ -399,7 +423,9 @@ size_t usearch_b200_profile_phases_n(usearch_index_t index, int enable, uint64_t
 /* Tuning knobs of the search launch for this handle ("stage_sets", "warps_per_sm", "prefilter" = 0 | 1: judge layer-0
  * candidates of cos / ip f32 on their int8 shadow first, on by default; "heap_head" = an upper bound on the candidate-heap
  * entries kept in shared memory, rounded down to an even number >= 2, the rest go to HBM; 0 = as planned), and
- * "get_chunk_rows" = rows per chunk of usearch_b200_get_many (0 = 64 MB of output); results never depend on them.
+ * "get_chunk_rows" = rows per chunk of usearch_b200_get_many (0 = 64 MB of output), and "group_bitmap_mb" = the MB of
+ * key-set bitmap rows one launch of usearch_b200_grouped_filtered_search_many may use (default 1024, at least one row
+ * is always used); results never depend on them.
  * Returns 0, or -1 for an unknown knob. */
 int usearch_b200_tune(usearch_index_t index, char const* knob, int value);
 /* The launch plan a search of `count` neighbours gets under the current knobs, for a loaded index. `out16` receives:

@@ -298,6 +298,27 @@ class index_dense_t {
                                                  keys, distances, counts, computed_distances, visited_members, cuda_stream, &e);
         return e;
     }
+    /* query i filtered by set groups[i]: set g is set_keys[offsets[g] .. offsets[g + 1]] (usearch_b200_grouped_filtered_search_many) */
+    template <typename scalar_at>
+    error_t grouped_filtered_search(scalar_at const* queries, std::size_t queries_count, std::size_t queries_stride, std::size_t wanted, std::uint32_t const* groups, std::uint64_t const* offsets, std::size_t sets_count,
+                                    vector_key_t const* set_keys, vector_key_t* keys, distance_t* distances, std::size_t* counts,
+                                    std::uint64_t* computed_distances = nullptr, std::uint64_t* visited_members = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_filtered_search_many(handle_, queries, queries_count, queries_stride, scalar_kind<scalar_at>(), wanted, groups, offsets,
+                                                  sets_count, set_keys, keys, distances, counts, computed_distances, visited_members, &e);
+        return e;
+    }
+    error_t grouped_filtered_search_device(void const* queries, std::size_t queries_count, std::size_t queries_stride, std::size_t wanted,
+                                           std::uint32_t const* groups, std::uint64_t const* offsets, std::size_t sets_count,
+                                           vector_key_t const* set_keys, vector_key_t* keys, distance_t* distances, std::uint32_t* counts,
+                                           std::uint32_t* computed_distances = nullptr, std::uint32_t* visited_members = nullptr,
+                                           void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_filtered_search_many_device(handle_, queries, queries_count, queries_stride, wanted, groups, offsets,
+                                                         sets_count, set_keys, keys, distances, counts, computed_distances,
+                                                         visited_members, cuda_stream, &e);
+        return e;
+    }
     /* index_dense.hpp:1595-1608, the live keys in slot order */
     void export_keys(vector_key_t* keys, std::size_t offset, std::size_t limit) const {
         usearch_b200_export_keys(handle_, offset, limit, keys, nullptr);

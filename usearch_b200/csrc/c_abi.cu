@@ -179,8 +179,10 @@ usearch_index_t usearch_init(usearch_init_options_t* options, usearch_error_t* e
 
 void usearch_free(usearch_index_t index, usearch_error_t*) { delete as_index(index); }
 
-size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table counts once it exists */
-    return as_index(index)->hbm_bytes + as_index(index)->key_table.cells.capacity * sizeof(key_cell_t);
+size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table and the grouped filter's
+                                                                        bitmap rows count once they exist */
+    frozen_index_t const* ix = as_index(index);
+    return ix->hbm_bytes + ix->key_table.cells.capacity * sizeof(key_cell_t) + ix->group_bits.capacity * sizeof(uint32_t);
 }
 
 char const* usearch_hardware_acceleration(usearch_index_t, usearch_error_t*) { return "sm_90a"; }
@@ -404,6 +406,46 @@ void usearch_b200_filtered_search_many_device(usearch_index_t index, void const*
         return ix->filtered_search_device(queries, queries_count, queries_stride, count, allowed_keys, allowed_count, keys, distances,
                                           counts, computed_distances, visited_members,
                                           cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
+    }));
+}
+
+/* grouped filtered search (grouped_filter.cu): query i filtered by key set groups[i] of a CSR list of sets */
+size_t usearch_b200_grouped_filtered_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                 size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                 uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                 usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                 size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
+                                                 usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    uint32_t qs = scalar_to_char(query_kind);
+    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
+    std::vector<size_t> own(counts ? 0 : queries_count);
+    size_t* const found = counts ? counts : own.data();
+    if (char const* e = guarded([&] {
+            return ix->grouped_filtered_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count, set_keys,
+                                                    keys, distances, found, computed_distances, visited_members);
+        })) {
+        set_error(error, e);
+        return 0;
+    }
+    size_t total = 0;
+    for (size_t i = 0; i < queries_count && count; ++i) total += found[i];
+    return total;
+}
+
+void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                      size_t queries_stride, size_t count, uint32_t const* groups,
+                                                      uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                      usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                      uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
+                                                      usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        return ix->grouped_filtered_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
+                                                  keys, distances, counts, computed_distances, visited_members,
+                                                  cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
     }));
 }
 
@@ -803,6 +845,7 @@ int usearch_b200_tune(usearch_index_t index, char const* knob, int value) {
     else if (!std::strcmp(knob, "prefilter")) ix->tune.prefilter = value;
     else if (!std::strcmp(knob, "heap_head")) ix->tune.heap_head = value;
     else if (!std::strcmp(knob, "get_chunk_rows")) ix->tune.get_chunk_rows = value;
+    else if (!std::strcmp(knob, "group_bitmap_mb")) ix->tune.group_bitmap_mb = value;
     else return -1;
     return 0;
 }

@@ -128,6 +128,12 @@ struct search_args_t {
     /* optional introspection: PHASE_COUNTERS counters summed over all queries (lane 0 clock64 deltas and counts), in
      * the order of include/usearch_b200.h (usearch_b200_profile_phases, usearch_b200_profile_phases_n) */
     unsigned long long* phase_cycles = nullptr;
+    /* grouped filtered search (GROUPED kernels only): `allow_bits` holds one row of `allow_words` words per group of the
+     * launch, and query qi tests row allow_groups[qi] - allow_group_base. Appended last, so that the parameter offsets the
+     * other kernels read stay where they were. */
+    uint32_t const* allow_groups = nullptr;
+    uint32_t allow_group_base = 0;
+    uint32_t allow_words = 0;
 };
 constexpr uint32_t PHASE_COUNTERS = 21;
 

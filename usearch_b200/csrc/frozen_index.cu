@@ -66,6 +66,7 @@ void frozen_index_t::release_device() {
     host_keys.clear();
     key_map.clear();
     key_table = key_table_t{};
+    group_bits = device_buffer_t<uint32_t>{};
     keys_generation += 1;
 }
 
@@ -382,7 +383,8 @@ char const* frozen_index_t::save_blob(uint8_t* out, size_t length) const {
 /*  launch planning                                                                               */
 /* ---------------------------------------------------------------------------------------------- */
 
-char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, launch_plan_t& pl, uint32_t ef_override) const {
+char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, launch_plan_t& pl, uint32_t ef_override,
+                                 bool grouped) const {
     uint32_t ef = (uint32_t)(expansion_search ? expansion_search : 64); /* index.hpp:3029-3030 */
     ef = std::max(ef, k);                                               /* index.hpp:3052 */
     if (ef_override) ef = ef_override; /* the builder searches with expansion_add (index.hpp:2854) */
@@ -507,7 +509,7 @@ char const* frozen_index_t::plan(uint32_t k, uint32_t visited_cap_override, laun
     }
 
     int per_sm = 0;
-    CU(search_occupancy(d, &per_sm, pl.smem_per_block));
+    CU(search_occupancy(d, &per_sm, pl.smem_per_block, grouped));
     if (per_sm < 1) return "Kernel does not fit on an SM";
     per_sm = std::min<int>(per_sm, (int)pl.warps_per_sm_target);
     pl.blocks = per_sm * stream.sm_count;
@@ -637,7 +639,8 @@ char const* frozen_index_t::search_finish() {
 }
 
 /* scratch overflow (h_status holds the status words of the launch described by `a`): rerun just those queries with 8x
- * larger tables until they fit */
+ * larger tables until they fit. The scan covers query ids 0 .. a.nq-1: a caller that launched through `query_list` passes
+ * `a.nq` as the id range, with every word outside the launch already STATUS_OK. */
 char const* frozen_index_t::retry_overflowed(search_args_t const& a, bool maxed, cudaStream_t s) {
     size_t const nq = a.nq, k = a.k;
     int const wpb = search_warps_per_block();
@@ -649,7 +652,7 @@ char const* frozen_index_t::retry_overflowed(search_args_t const& a, bool maxed,
         if (maxed) return "Search scratch overflow that full-size scratch could not fix";
         scale *= 8;
         launch_plan_t rp;
-        if (char const* e = plan((uint32_t)k, (uint32_t)std::min<uint64_t>(scale, 1u << 30), rp)) return e;
+        if (char const* e = plan((uint32_t)k, (uint32_t)std::min<uint64_t>(scale, 1u << 30), rp, 0, a.allow_groups != nullptr)) return e;
         maxed = rp.maxed;
         size_t const bytes_per_warp = (size_t)rp.visited_words_per_warp() * 4 + (size_t)rp.heap_spill_cap * 8;
         size_t max_warps = std::max<size_t>(wpb, ((size_t)2 << 30) / bytes_per_warp / wpb * wpb);
@@ -664,6 +667,7 @@ char const* frozen_index_t::retry_overflowed(search_args_t const& a, bool maxed,
         r.out_keys = a.out_keys; r.out_dists = a.out_dists; r.out_counts = a.out_counts;
         r.out_computed = a.out_computed; r.out_visited = a.out_visited; r.status = a.status;
         r.allow_bits = a.allow_bits; r.cluster_end_level = a.cluster_end_level; r.phase_cycles = a.phase_cycles;
+        r.allow_groups = a.allow_groups; r.allow_group_base = a.allow_group_base; r.allow_words = a.allow_words;
         r.nq = (uint32_t)failed.size();
         r.query_list = retry_list.ptr;
         CU(cudaMemsetAsync(work_counter.ptr, 0, 8, s));

@@ -24,7 +24,7 @@ namespace usearch_b200 {
 
 /* kernel entry points (search_kernel.cu) */
 cudaError_t search_launch(device_index_t const& ix, search_args_t const& a, int blocks, size_t smem, cudaStream_t stream);
-cudaError_t search_occupancy(device_index_t const& ix, int* blocks_per_sm, size_t smem);
+cudaError_t search_occupancy(device_index_t const& ix, int* blocks_per_sm, size_t smem, bool grouped = false);
 bool search_supported(uint32_t metric, uint32_t scalar);
 int search_warps_per_block();
 bool search_is_staged(device_index_t const& ix);
@@ -126,6 +126,8 @@ struct frozen_index_t {
         int heap_head = env_int("USEARCH_B200_HEAP_HEAD", 0);       /* 0 = as planned, else an upper bound on the heap
                                                                        entries kept in shared memory (even, >= 2) */
         int get_chunk_rows = env_int("USEARCH_B200_GET_CHUNK_ROWS", 0); /* rows per chunk of get_many; 0 = 64 MB of output */
+        int group_bitmap_mb = env_int("USEARCH_B200_GROUP_BITMAP_MB", 1024); /* grouped filtered search: bitmap rows per
+                                                                               round fill at most this many MB (at least one row) */
         static int env_int(char const* name, int fallback) {
             char const* v = std::getenv(name);
             return v ? std::atoi(v) : fallback;
@@ -224,8 +226,26 @@ struct frozen_index_t {
                                        size_t allowed_count, uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed,
                                        uint32_t* d_visited, cudaStream_t s);
 
+    /* grouped_filter.cu: a batch whose query i is filtered by key set groups[i], the sets given as CSR (offsets[G + 1] into
+     * set_keys), every pointer in device memory. One bitmap row per set, built from the key table; rows of as many sets
+     * as `group_bitmap_mb` allows per launch. */
+    device_buffer_t<uint32_t> group_bits; /* the rows of one round; counted by memory_usage */
+    device_buffer_t<uint32_t> group_order, group_sorted, group_ids, group_bounds, group_flag;
+    device_buffer_t<uint8_t> group_sort_temp;
+    device_buffer_t<uint64_t> group_offsets; /* the host entry's upload of `offsets` (its keys go to `allowed_keys`) */
+    device_buffer_t<uint32_t> group_upload;   /* ... and of `groups` */
+    char const* grouped_filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                               uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
+                                               float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                               cudaStream_t s);
+    char const* grouped_filtered_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                             uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
+                                             uint64_t* keys, float* dists, size_t* counts, uint64_t* computed, uint64_t* visited);
+
     /* searches */
-    char const* plan(uint32_t k, uint32_t visited_cap_override, launch_plan_t& plan, uint32_t ef_override = 0) const;
+    /* grouped: plan for the GROUPED kernel (its occupancy) */
+    char const* plan(uint32_t k, uint32_t visited_cap_override, launch_plan_t& plan, uint32_t ef_override = 0,
+                     bool grouped = false) const;
     char const* prepare_launch(launch_plan_t const& pl, size_t warps, search_args_t& a, cudaStream_t s);
     char const* search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t* d_keys, float* d_dists,
                               uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles, cudaStream_t stream, bool defer = false);

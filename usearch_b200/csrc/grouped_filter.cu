@@ -1,0 +1,260 @@
+/*
+ *  grouped_filter.cu — filtered search where every query brings its own key set: query i is searched as
+ *  filtered_search(queries[i], k, set_keys[offsets[g] .. offsets[g + 1]]) with g = groups[i], all in one launch.
+ *
+ *  Each set becomes one bitmap row over slots (ceil(size / 32) words), the row allow_bits_kernel would build for it: one
+ *  thread per (set, key) entry walks the key -> slot table (device_keys.h) and sets the bit of every slot it finds, so the
+ *  cost is O(total keys), never O(slots x sets). The GROUPED search kernels test row groups[qi] where the single-set
+ *  kernels test their one bitmap. When the rows of all sets do not fit the `group_bitmap_mb` budget, the sets are served
+ *  in rounds of consecutive set ids, each round's queries a contiguous slice of the query ids sorted by set.
+ */
+#include <cub/device/device_radix_sort.cuh>
+
+#include <algorithm>
+
+#include "cuda_check.h"
+#include "device_keys.h"
+#include "frozen_index.h"
+
+namespace usearch_b200 {
+
+namespace {
+
+char const* const ERR_SHARDED = "Grouped filtered search does not serve a sharded handle: it holds one shard of its index";
+char const* const ERR_NO_SETS = "A batch of queries needs at least one key set";
+char const* const ERR_GROUP = "A query's key set index is out of range";
+char const* const ERR_OFFSETS = "Key set offsets must start at 0 and never decrease";
+
+enum : uint32_t { BAD_GROUP = 1, BAD_OFFSETS = 2 };
+
+unsigned grid_for(size_t items, int sm_count) { return (unsigned)std::max<size_t>(1, std::min<size_t>((items + 255) / 256, (size_t)sm_count * 16)); }
+
+__global__ void grouped_validate_kernel(uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count, uint32_t* flag) {
+    size_t const n = max(nq, group_count);
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        if (i < nq && groups[i] >= group_count) atomicOr(flag, (uint32_t)BAD_GROUP);
+        if (i < group_count && offsets[i + 1] < offsets[i]) atomicOr(flag, (uint32_t)BAD_OFFSETS);
+        if (i == 0 && offsets[0] != 0) atomicOr(flag, (uint32_t)BAD_OFFSETS);
+    }
+}
+
+/* rows[(g - g0) * words ..] |= the slots of every key of set g, for g0 <= g < g1; the rows start zeroed. The free key
+ * allows the removed slots, as allow_bits_kernel's search of keys[] does (the deleted bits reject them first anyway). */
+__global__ void grouped_bits_kernel(key_cell_t const* cells, uint64_t mask, uint64_t const* offsets, uint64_t const* set_keys, uint32_t g0,
+                                    uint32_t g1, uint64_t free_key, uint32_t const* deleted_bits, uint32_t size, uint32_t words,
+                                    uint32_t* rows) {
+    uint64_t const begin = offsets[g0], end = offsets[g1];
+    for (uint64_t e = begin + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < end; e += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t lo = g0 + 1, hi = g1; /* the first set past entry e: offsets[lo] > e */
+        while (lo < hi) {
+            uint32_t const mid = (lo + hi) >> 1;
+            if (offsets[mid] > e) hi = mid;
+            else lo = mid + 1;
+        }
+        uint32_t* const row = rows + (size_t)(lo - 1 - g0) * words;
+        uint64_t const key = set_keys[e];
+        if (key == free_key) {
+            if (deleted_bits)
+                for (uint32_t w = 0; w < words; ++w) {
+                    uint32_t bits = deleted_bits[w];
+                    if (w == words - 1 && (size & 31)) bits &= (1u << (size & 31)) - 1u;
+                    if (bits) atomicOr(row + w, bits);
+                }
+            continue;
+        }
+        key_table_for_each(cells, mask, key, [&](uint32_t s) { atomicOr(row + (s >> 5), 1u << (s & 31)); });
+    }
+}
+
+__global__ void iota_u32_kernel(uint32_t* out, size_t n) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) out[i] = (uint32_t)i;
+}
+
+/* bounds[r] = the first position of `sorted` holding a set id >= r * per_round, for r <= rounds */
+__global__ void round_bounds_kernel(uint32_t const* sorted, uint32_t nq, uint32_t per_round, uint32_t rounds, uint32_t* bounds) {
+    uint32_t const r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r > rounds) return;
+    uint64_t const first = (uint64_t)r * per_round;
+    uint32_t lo = 0, hi = nq;
+    while (lo < hi) {
+        uint32_t const mid = (lo + hi) >> 1;
+        if (sorted[mid] < first) lo = mid + 1;
+        else hi = mid;
+    }
+    bounds[r] = lo;
+}
+
+} // namespace
+
+char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
+                                                           uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                           uint64_t const* set_keys, uint64_t* d_keys, float* d_dists,
+                                                           uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                                           cudaStream_t s) {
+    if (shards) return ERR_SHARDED;
+    if (char const* e = ensure_context()) return e;
+    if (nq == 0 || k == 0) return nullptr;
+    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
+    if (group_count == 0) return ERR_NO_SETS;
+    if (group_count >= 0xFFFFFFFFull) return "Too many key sets in one call";
+
+    /* every refusal comes before the first write to an output */
+    if (char const* e = group_flag.reserve(1)) return e;
+    CU(cudaMemsetAsync(group_flag.ptr, 0, 4, s));
+    grouped_validate_kernel<<<grid_for(std::max(nq, group_count), stream.sm_count), 256, 0, s>>>(groups, nq, offsets, group_count,
+                                                                                                 group_flag.ptr);
+    CU(cudaGetLastError());
+    kernel_launches += 1;
+    uint32_t flag = 0;
+    CU(cudaMemcpyAsync(&flag, group_flag.ptr, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (flag & BAD_GROUP) return ERR_GROUP;
+    if (flag & BAD_OFFSETS) return ERR_OFFSETS;
+
+    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
+        CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
+        CU(cudaStreamSynchronize(s));
+        return nullptr;
+    }
+    if (char const* e = ensure_key_table(s)) return e;
+    uint32_t const words = (uint32_t)((size + 31) / 32);
+    size_t const budget = (size_t)std::max(tune.group_bitmap_mb, 0) << 20;
+    size_t const per_round = std::min<size_t>(std::max<size_t>(budget / ((size_t)words * 4), 1), group_count);
+    size_t const rounds = (group_count + per_round - 1) / per_round;
+    if (char const* e = group_bits.reserve(per_round * words)) return e;
+
+    launch_plan_t pl;
+    if (char const* e = plan((uint32_t)k, 0, pl, 0, true)) return e;
+    int const wpb = search_warps_per_block();
+    if (char const* e = h_status.reserve(nq)) return e;
+    if (char const* e = status.reserve(nq)) return e;
+    /* the retry of a round scans every query id: the words of the other rounds' queries must read STATUS_OK */
+    CU(cudaMemsetAsync(status.ptr, 0, nq * 4, s));
+    if (profile_phases)
+        if (char const* e = phase_cycles.reserve(PHASE_COUNTERS)) return e;
+
+    /* the sets [g0, g1) into rows, then their queries: `items` work items, through `list` when it is not NULL */
+    auto round = [&](uint32_t g0, uint32_t g1, uint32_t const* list, size_t items) -> char const* {
+        CU(cudaMemsetAsync(group_bits.ptr, 0, (size_t)(g1 - g0) * words * 4, s));
+        grouped_bits_kernel<<<stream.sm_count * 16, 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, set_keys, g0, g1,
+                                                                 free_key, d.deleted_bits, (uint32_t)size, words, group_bits.ptr);
+        CU(cudaGetLastError());
+        kernel_launches += 1;
+        int const blocks = (int)std::min<size_t>((size_t)pl.blocks, (items + wpb - 1) / wpb);
+        search_args_t a;
+        if (char const* e = prepare_launch(pl, (size_t)blocks * wpb, a, s)) return e;
+        a.queries = static_cast<uint8_t const*>(d_queries);
+        a.query_stride = stride;
+        a.nq = (uint32_t)items;
+        a.query_list = list;
+        a.k = (uint32_t)k;
+        a.out_keys = d_keys;
+        a.out_dists = d_dists;
+        a.out_counts = d_counts;
+        a.out_computed = d_computed;
+        a.out_visited = d_visited;
+        a.status = status.ptr;
+        a.allow_bits = group_bits.ptr;
+        a.allow_groups = groups;
+        a.allow_group_base = g0;
+        a.allow_words = words;
+        if (profile_phases) a.phase_cycles = phase_cycles.ptr;
+        CU(cudaMemsetAsync(work_counter.ptr, 0, 8, s));
+        CU(cudaEventRecord(ev_begin, s));
+        CU(search_launch(d, a, blocks, pl.smem_per_block, s));
+        CU(cudaEventRecord(ev_end, s));
+        kernel_launches += 1;
+        CU(cudaMemcpyAsync(h_status.ptr, status.ptr, nq * 4, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        CU(cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end));
+        search_args_t every = a; /* the failed queries of this round, by query id */
+        every.nq = (uint32_t)nq;
+        return retry_overflowed(every, pl.maxed, s);
+    };
+    if (rounds == 1) return round(0, (uint32_t)group_count, nullptr, nq);
+
+    /* query ids sorted by set: round r serves the contiguous slice of ids whose sets lie in its range */
+    if (char const* e = group_ids.reserve(nq)) return e;
+    if (char const* e = group_order.reserve(nq)) return e;
+    if (char const* e = group_sorted.reserve(nq)) return e;
+    if (char const* e = group_bounds.reserve(rounds + 1)) return e;
+    iota_u32_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(group_ids.ptr, nq);
+    CU(cudaGetLastError());
+    int end_bit = 1;
+    while (end_bit < 32 && (group_count - 1) >> end_bit) ++end_bit;
+    size_t temp_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, groups, group_sorted.ptr, group_ids.ptr, group_order.ptr, (int)nq, 0, end_bit, s));
+    if (char const* e = group_sort_temp.reserve(temp_bytes)) return e;
+    CU(cub::DeviceRadixSort::SortPairs(group_sort_temp.ptr, temp_bytes, groups, group_sorted.ptr, group_ids.ptr, group_order.ptr, (int)nq, 0,
+                                       end_bit, s));
+    round_bounds_kernel<<<(unsigned)((rounds + 1 + 255) / 256), 256, 0, s>>>(group_sorted.ptr, (uint32_t)nq, (uint32_t)per_round,
+                                                                             (uint32_t)rounds, group_bounds.ptr);
+    CU(cudaGetLastError());
+    kernel_launches += 3;
+    std::vector<uint32_t> bounds(rounds + 1);
+    CU(cudaMemcpyAsync(bounds.data(), group_bounds.ptr, (rounds + 1) * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    for (size_t r = 0; r < rounds; ++r) {
+        if (bounds[r + 1] == bounds[r]) continue; /* no query asks for these sets */
+        uint32_t const g0 = (uint32_t)(r * per_round), g1 = (uint32_t)std::min(group_count, (r + 1) * per_round);
+        if (char const* e = round(g0, g1, group_order.ptr + bounds[r], bounds[r + 1] - bounds[r])) return e;
+    }
+    return nullptr;
+}
+
+/* host queries of any kind, host sets and host outputs: validated here (the offsets size the upload), uploaded, and run
+ * through the device path */
+char const* frozen_index_t::grouped_filtered_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                         uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                         uint64_t const* set_keys, uint64_t* keys, float* dists, size_t* counts_out,
+                                                         uint64_t* computed_out, uint64_t* visited_out) {
+    std::lock_guard<std::mutex> lock(mutex);
+    if (shards) return ERR_SHARDED;
+    if (nq == 0 || k == 0) return nullptr;
+    if (group_count == 0) return ERR_NO_SETS;
+    if (offsets[0] != 0) return ERR_OFFSETS;
+    for (size_t g = 0; g < group_count; ++g)
+        if (offsets[g + 1] < offsets[g]) return ERR_OFFSETS;
+    for (size_t i = 0; i < nq; ++i)
+        if (groups[i] >= group_count) return ERR_GROUP;
+    if (!loaded || d.n == 0) { /* as search_host answers on an empty index */
+        for (size_t i = 0; i < nq; ++i) {
+            for (size_t j = 0; j < k; ++j) { keys[i * k + j] = 0; reinterpret_cast<uint32_t*>(dists)[i * k + j] = SNAN_BITS; }
+            if (counts_out) counts_out[i] = 0;
+            if (computed_out) computed_out[i] = 0;
+            if (visited_out) visited_out[i] = 0;
+        }
+        return nullptr;
+    }
+    if (char const* e = ensure_context()) return e;
+    size_t const vs = d.vec_stride ? d.vec_stride : 16, total = offsets[group_count];
+    if (char const* e = queries.reserve(nq * vs)) return e;
+    if (char const* e = out_keys.reserve(nq * k)) return e;
+    if (char const* e = out_dists.reserve(nq * k)) return e;
+    if (char const* e = counts_reserve_all(nq)) return e;
+    if (char const* e = group_upload.reserve(nq)) return e;
+    if (char const* e = group_offsets.reserve(group_count + 1)) return e;
+    if (char const* e = allowed_keys.reserve(std::max<size_t>(total, 1))) return e;
+    if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
+    CU(cudaMemcpyAsync(group_upload.ptr, groups, nq * 4, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(group_offsets.ptr, offsets, (group_count + 1) * 8, cudaMemcpyHostToDevice, stream));
+    if (total) CU(cudaMemcpyAsync(allowed_keys.ptr, set_keys, total * 8, cudaMemcpyHostToDevice, stream));
+    if (char const* e = grouped_filtered_search_device(queries.ptr, nq, vs, k, group_upload.ptr, group_offsets.ptr, group_count,
+                                                       allowed_keys.ptr, out_keys.ptr, out_dists.ptr, this->counts.ptr, computed.ptr,
+                                                       cycles.ptr, stream))
+        return e;
+    CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_counts.ptr, this->counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_computed.ptr, computed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_cycles.ptr, cycles.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    for (size_t i = 0; i < nq; ++i) {
+        if (counts_out) counts_out[i] = h_counts.ptr[i];
+        if (computed_out) computed_out[i] = h_computed.ptr[i];
+        if (visited_out) visited_out[i] = h_cycles.ptr[i];
+    }
+    return nullptr;
+}
+
+} // namespace usearch_b200

@@ -684,15 +684,26 @@ __device__ __forceinline__ bool slot_allowed(device_index_t const& ix, search_ar
     return true;
 }
 
+/* the same predicate with the query's own bitmap row (grouped filtered search) */
+__device__ __forceinline__ bool slot_allowed_row(device_index_t const& ix, uint32_t const* row, uint32_t s) {
+    if (ix.deleted_bits && ((ix.deleted_bits[s >> 5] >> (s & 31)) & 1u)) return false;
+    return (row[s >> 5] >> (s & 31)) & 1u;
+}
+
 /* ---- one query ------------------------------------------------------------------------------ */
 
-template <class M, bool STAGED, bool INSERT>
+template <class M, bool STAGED, bool INSERT, bool GROUPED>
 __device__ __forceinline__ void search_one(device_index_t const& ix, search_args_t const& a, uint32_t qi, uint32_t out_row,
                                            int const bl_arg, warp_ctx_t& w, heap_t const& heap, uint32_t* visited, int lane) {
     uint32_t const k = a.k, ef = a.ef;
     /* INSERT mode: search_to_insert_ (index.hpp:4010-4079) on level `bl` — no predicate, slots out. A template
      * parameter, so that the plain search kernels compile to the code they had before the builder existed. */
     constexpr bool insert = INSERT;
+    /* GROUPED: query qi's predicate is the bitmap row of its own group, resolved once here (by query id, never by work
+     * item, so retries and rounds launched through `query_list` find the same row). A template parameter for the same
+     * reason as INSERT. */
+    uint32_t const* const group_row =
+        GROUPED ? a.allow_bits + (size_t)(a.allow_groups[qi] - a.allow_group_base) * a.allow_words : nullptr;
     int const bl = INSERT ? bl_arg : 0;
     uint32_t const width = bl == 0 ? ix.m0 : ix.m; /* list capacity on the searched level */
     auto row_of = [&](uint32_t slot) -> uint32_t const* {
@@ -853,7 +864,8 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
             /* cluster(): the closest member at that level is the whole answer, predicate ignored (index.hpp:3122) */
             /* search_to_update_ (index.hpp:4086-4168): a reused slot is searched from and expanded, but never
              * enters its own `top`. For an appended member no list reaches its slot, so the test never fires. */
-            bool allowed = cluster || (insert ? closest != qi : slot_allowed(ix, a, closest));
+            bool allowed = cluster || (insert ? closest != qi
+                                                   : GROUPED ? slot_allowed_row(ix, group_row, closest) : slot_allowed(ix, a, closest));
             if (allowed) {
                 if (topreg) {
                     if (lane == 0) { rtd[0] = radius; rts[0] = closest; }
@@ -1016,7 +1028,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
                         heap.push(heap_size, cand_t{d, s}, lane);
                         heap_size += 1;
                         if (prof) { n_push += 1; max_heap = max(max_heap, heap_size); }
-                        bool allowed = insert ? s != qi : slot_allowed(ix, a, s);
+                        bool allowed = insert ? s != qi : GROUPED ? slot_allowed_row(ix, group_row, s) : slot_allowed(ix, a, s);
                         if (allowed) {
                             if (topreg) {
                                 top_insert_reg(rtd, rts, top_size, ef, d, s, lane);
@@ -1130,7 +1142,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
 
 /* MIN_CTAS: resident CTAs (= warps) per SM the register allocation must allow: 8 for the staged f32 kernel (its 16
  * accumulators and the register-resident `top` want ~220 registers), 16 for everything else (see the dispatch below). */
-template <class M, bool STAGED, int MIN_CTAS = (STAGED ? 8 : 16), bool INSERT = false>
+template <class M, bool STAGED, int MIN_CTAS = (STAGED ? 8 : 16), bool INSERT = false, bool GROUPED = false>
 __global__ void __launch_bounds__(THREADS, MIN_CTAS) hnsw_search_kernel(__grid_constant__ device_index_t const ix,
                                                               __grid_constant__ search_args_t const a) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -1162,7 +1174,7 @@ __global__ void __launch_bounds__(THREADS, MIN_CTAS) hnsw_search_kernel(__grid_c
         /* INSERT mode: one output row per work item (the same member is searched once per level) */
         uint32_t const out_row = INSERT ? item : qi;
         int const bl = INSERT ? (int)a.task_levels[item] : 0;
-        search_one<M, STAGED, INSERT>(ix, a, qi, out_row, bl, w, heap, visited, lane);
+        search_one<M, STAGED, INSERT, GROUPED>(ix, a, qi, out_row, bl, w, heap, visited, lane);
     }
 }
 
@@ -1311,12 +1323,20 @@ cudaError_t search_compute_shadow(device_index_t const& ix, float const* norms, 
  *    i8, >= 256 B               STAGED compiled for 16 resident warps per SM, one stage set up to 2 KB: a hop moves few
  *                               bytes, so resident warps matter more than double buffering
  *    b1, and anything < 256 B   DIRECT (16-byte chunks through registers)
- *  Every one of them also exists as an INSERT-mode kernel for the builder.
+ *  Every one of them also exists as an INSERT-mode kernel for the builder, and as a GROUPED kernel for grouped filtered
+ *  search.
  */
 template <class M, bool STAGED, int MIN_CTAS>
 static cudaError_t launch_k(device_index_t const& ix, search_args_t const& a, int blocks, size_t smem, cudaStream_t stream) {
     if (a.out_slots) { /* INSERT mode (builder.cu) */
         auto kernel = hnsw_search_kernel<M, STAGED, MIN_CTAS, true>;
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        kernel<<<blocks, THREADS, smem, stream>>>(ix, a);
+        return cudaGetLastError();
+    }
+    if (a.allow_groups) { /* grouped filtered search: a bitmap row per query's group */
+        auto kernel = hnsw_search_kernel<M, STAGED, MIN_CTAS, false, true>;
         cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         kernel<<<blocks, THREADS, smem, stream>>>(ix, a);
@@ -1329,8 +1349,9 @@ static cudaError_t launch_k(device_index_t const& ix, search_args_t const& a, in
     return cudaGetLastError();
 }
 
-template <class M, bool STAGED, int MIN_CTAS> static cudaError_t occupancy_k(int* blocks_per_sm, size_t smem) {
-    auto kernel = hnsw_search_kernel<M, STAGED, MIN_CTAS, false>; /* the INSERT twin needs no more registers */
+template <class M, bool STAGED, int MIN_CTAS> static cudaError_t occupancy_k(int* blocks_per_sm, size_t smem, bool grouped) {
+    /* the INSERT twin needs no more registers; the GROUPED one is asked for itself */
+    auto kernel = grouped ? hnsw_search_kernel<M, STAGED, MIN_CTAS, false, true> : hnsw_search_kernel<M, STAGED, MIN_CTAS, false>;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kernel, THREADS, smem);
@@ -1399,9 +1420,9 @@ cudaError_t search_launch(device_index_t const& ix, search_args_t const& a, int 
     FOR_METRIC(launch_k, (ix, a, blocks, smem, stream))
 }
 
-cudaError_t search_occupancy(device_index_t const& ix, int* blocks_per_sm, size_t smem) {
+cudaError_t search_occupancy(device_index_t const& ix, int* blocks_per_sm, size_t smem, bool grouped) {
     bool const staged = search_is_staged(ix);
-    FOR_METRIC(occupancy_k, (blocks_per_sm, smem))
+    FOR_METRIC(occupancy_k, (blocks_per_sm, smem, grouped))
 }
 
 bool search_supported(uint32_t metric, uint32_t scalar) {

@@ -60,7 +60,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_indexes_size", "usearch_b200_indexes_search_many", "usearch_b200_indexes_last_ms", "usearch_b200_merge_into",
     "usearch_b200_get_many", "usearch_b200_export_keys", "usearch_b200_export_keys_at", "usearch_b200_copy",
     "usearch_b200_levels_stats", "usearch_b200_multi", "usearch_b200_count_many_device", "usearch_b200_get_many_device",
-    "usearch_b200_filtered_search_many_device",
+    "usearch_b200_filtered_search_many_device", "usearch_b200_grouped_filtered_search_many",
+    "usearch_b200_grouped_filtered_search_many_device",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -119,6 +120,14 @@ def load_library() -> C.CDLL:
                                                              C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                                              C.c_void_p, C.c_void_p, C.c_void_p, err]
     lib.usearch_b200_search_many_finish.argtypes = [C.c_void_p, err]
+    lib.usearch_b200_grouped_filtered_search_many.restype = C.c_size_t
+    lib.usearch_b200_grouped_filtered_search_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t,
+                                                              C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_grouped_filtered_search_many_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                                     C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                     err]
     lib.usearch_b200_tune.restype = C.c_int
     lib.usearch_b200_tune.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
     lib.usearch_b200_launch_plan.restype = C.c_int
@@ -737,6 +746,59 @@ class Index:
         """`filtered_search` (index_dense.hpp:774-779) for the predicate "key in allowed_keys"."""
         return self.search(vectors, count, stats=True, _allowed=np.ascontiguousarray(allowed_keys, dtype=np.uint64))
 
+    def grouped_filtered_search(self, vectors: np.ndarray, count: int, key_sets, groups=None) -> Union[Matches, BatchMatches]:
+        """`filtered_search` with a key set per query, as one launch: row i equals
+        ``filtered_search(vectors[i], count, key_sets[groups[i]])``, counters included (`last_computed` / `last_visited`).
+        `key_sets` is a sequence of key iterables or arrays; ``groups=None`` gives query i the set i."""
+        vectors = np.asarray(vectors)
+        single = vectors.ndim == 1
+        if single:
+            vectors = vectors[None, :]
+        if vectors.ndim != 2:
+            raise ValueError("Expects a matrix or a vector")
+        nq = vectors.shape[0]
+        sets = []
+        for keys in key_sets:
+            if np.isscalar(keys):
+                raise ValueError("key_sets must be a sequence of key sets, not of keys")
+            keys = keys if isinstance(keys, np.ndarray) else np.asarray(list(keys))
+            sets.append(np.ascontiguousarray(keys.reshape(-1), dtype=np.uint64))
+        if groups is None:
+            if len(sets) != nq:
+                raise ValueError("Without groups, key_sets needs one set per query")
+            groups = np.arange(nq, dtype=np.uint32)
+        else:
+            groups = np.asarray(groups)
+            if groups.shape != (nq,):
+                raise ValueError("groups needs one set index per query")
+            if nq and (groups.min() < 0 or groups.max() >= len(sets)):
+                raise ValueError("A query's key set index is out of range")
+            groups = np.ascontiguousarray(groups, dtype=np.uint32)
+        offsets = np.zeros(len(sets) + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum([len(keys) for keys in sets]) if sets else []
+        flat = np.concatenate(sets) if sets else np.zeros(0, dtype=np.uint64)
+        if not vectors.flags.c_contiguous and vectors.strides[1] != vectors.itemsize:
+            vectors = np.ascontiguousarray(vectors)
+        kind = self._kind_of(vectors)
+        keys = np.zeros((nq, count), dtype=np.uint64)
+        distances = np.zeros((nq, count), dtype=np.float32)
+        counts = np.zeros(nq, dtype=np.uint64)
+        computed = np.zeros(nq, dtype=np.uint64)
+        visited = np.zeros(nq, dtype=np.uint64)
+        err = C.c_char_p()
+        self._lib.usearch_b200_grouped_filtered_search_many(
+            self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count,
+            groups.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), len(sets), flat.ctypes.data_as(C.c_void_p),
+            keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
+            computed.ctypes.data_as(C.c_void_p), visited.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        self.last_computed, self.last_visited = computed, visited
+        vm, cd = int(visited.sum()), int(computed.sum())
+        if single:
+            n = int(counts[0])
+            return Matches(keys[0, :n], distances[0, :n], vm, cd)
+        return BatchMatches(keys, distances, counts, vm, cd)
+
     def cluster(self, vectors: np.ndarray, level: int = 1, *, stats: bool = False):
         """`index_dense_gt::cluster(vector, level)` (index_dense.hpp:788-793; index.hpp:3092-3125) for every row: the
         closest member on graph level `level` (levels above the top return the entry point; 0 behaves like 1).
@@ -828,7 +890,8 @@ class Index:
         return BatchMatches(keys, distances, counts, vm, cd)
 
     def tune(self, **knobs: int) -> None:
-        """Launch tuning knobs of this handle (stage_sets, warps_per_sm, prefilter, heap_head); results never change."""
+        """Launch tuning knobs of this handle (stage_sets, warps_per_sm, prefilter, heap_head, get_chunk_rows,
+        group_bitmap_mb); results never change."""
         for name, value in knobs.items():
             if self._lib.usearch_b200_tune(self._h, name.encode(), int(value)) != 0:
                 raise ValueError(f"unknown knob {name}")
@@ -953,6 +1016,18 @@ class Index:
                                                            allowed_count, keys_ptr, distances_ptr, counts_ptr,
                                                            computed_ptr or None, visited_ptr or None, stream or None,
                                                            C.byref(err))
+        _raise(err)
+
+    def grouped_filtered_search_device(self, queries_ptr: int, nq: int, stride: int, count: int, groups_ptr: int, offsets_ptr: int,
+                                       sets_count: int, set_keys_ptr: int, keys_ptr: int, distances_ptr: int, counts_ptr: int,
+                                       computed_ptr: int = 0, visited_ptr: int = 0, stream: int = 0) -> None:
+        """`grouped_filtered_search` on DEVICE memory: queries in the index's kind, `groups` (uint32 [nq]), `offsets`
+        (uint64 [sets_count + 1]) and `set_keys` (uint64), outputs laid out as in `search_device`."""
+        err = C.c_char_p()
+        self._lib.usearch_b200_grouped_filtered_search_many_device(self._h, queries_ptr, nq, stride, count, groups_ptr or None,
+                                                                   offsets_ptr or None, sets_count, set_keys_ptr or None, keys_ptr,
+                                                                   distances_ptr, counts_ptr, computed_ptr or None,
+                                                                   visited_ptr or None, stream or None, C.byref(err))
         _raise(err)
 
 
