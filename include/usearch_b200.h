@@ -360,6 +360,28 @@ void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, voi
                                                       uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                                       usearch_error_t* error);
 
+/* Exact filtered search: usearch_b200_grouped_filtered_search_many's sets and rows, but every query scans exactly the live
+ * entries whose key is in its set, as the reference's filtered_search(..., exact = true) does (index_dense.hpp:774-779,
+ * index.hpp:4251-4268): keys, distances and counts equal it, ties in the order of search(exact = true). A removed entry
+ * never counts, even when the free key is in the set; on a multi index every entry of a key counts. computed_distances[i]
+ * receives the number of entries query i measured (the live entries of its set). `groups` may be NULL when sets_count is 1:
+ * every query uses set 0. Each set becomes an ascending list of its slots, so the cost follows the sets' sizes, never
+ * slots x sets. Refusals as in usearch_b200_grouped_filtered_search_many. Buffers are HOST memory; queries may be of any
+ * kind. Returns the sum of counts. */
+size_t usearch_b200_grouped_filtered_exact_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                       size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                       uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                       usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                       size_t* counts, uint64_t* computed_distances, usearch_error_t* error);
+/* The same with DEVICE queries (in the index's kind; any stride), DEVICE groups, offsets, set keys and outputs, on
+ * `cuda_stream` (NULL = the handle's stream). The arguments are checked on the device before the search; the call returns
+ * when the outputs are complete. */
+void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                            size_t queries_stride, size_t count, uint32_t const* groups,
+                                                            uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                            usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                            uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error);
+
 /* The asynchronous pair. `enqueue` = the same arguments as usearch_b200_search_many_device, but it ONLY enqueues the
  * kernel on `cuda_stream` and returns; any number of batches may be in flight. `finish` waits for them, inspects the
  * per-query status words and re-runs, with larger scratch, the rare queries whose scratch overflowed; the outputs of

@@ -319,6 +319,70 @@ class index_dense_t {
                                                          visited_members, cuda_stream, &e);
         return e;
     }
+    /* the exact forms: every query scans exactly the live entries of its set (usearch_b200_grouped_filtered_exact_search_many);
+     * `groups` may be NULL with one set */
+    template <typename scalar_at>
+    error_t grouped_filtered_exact_search(scalar_at const* queries, std::size_t queries_count, std::size_t queries_stride,
+                                          std::size_t wanted, std::uint32_t const* groups, std::uint64_t const* offsets,
+                                          std::size_t sets_count, vector_key_t const* set_keys, vector_key_t* keys,
+                                          distance_t* distances, std::size_t* counts,
+                                          std::uint64_t* computed_distances = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_filtered_exact_search_many(handle_, queries, queries_count, queries_stride, scalar_kind<scalar_at>(), wanted,
+                                                        groups, offsets, sets_count, set_keys, keys, distances, counts,
+                                                        computed_distances, &e);
+        return e;
+    }
+    error_t grouped_filtered_exact_search_device(void const* queries, std::size_t queries_count, std::size_t queries_stride,
+                                                 std::size_t wanted, std::uint32_t const* groups, std::uint64_t const* offsets,
+                                                 std::size_t sets_count, vector_key_t const* set_keys, vector_key_t* keys,
+                                                 distance_t* distances, std::uint32_t* counts,
+                                                 std::uint32_t* computed_distances = nullptr, void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_filtered_exact_search_many_device(handle_, queries, queries_count, queries_stride, wanted, groups, offsets,
+                                                               sets_count, set_keys, keys, distances, counts, computed_distances,
+                                                               cuda_stream, &e);
+        return e;
+    }
+    /* index_dense.hpp:774-779. `exact`: predicate(key) is called once per live entry on the host and the entries it accepts
+     * are scanned on the device; otherwise the predicate goes to usearch_filtered_search, which cannot run a host callback
+     * on the device and reports so. `thread` is accepted and ignored. */
+    template <typename scalar_at, typename predicate_at>
+    search_result_t filtered_search(scalar_at const* vector, std::size_t wanted, predicate_at&& predicate, std::size_t /*thread*/ = 0,
+                                    bool exact = false) const {
+        search_result_t result;
+        if (!wanted) return result;
+        result.keys_.resize(wanted);
+        result.distances_.resize(wanted);
+        usearch_error_t error = nullptr;
+        if (!exact) {
+            /* the predicate's own constness is kept: `state` only carries its address back to the call */
+            typedef typename std::remove_reference<predicate_at>::type predicate_t;
+            struct trampoline_t {
+                static int call(vector_key_t key, void* state) { return (*static_cast<predicate_t*>(state))(key) ? 1 : 0; }
+            };
+            void* const state = const_cast<void*>(static_cast<void const*>(&predicate));
+            result.count = usearch_filtered_search(handle_, vector, scalar_kind<scalar_at>(), wanted, &trampoline_t::call, state,
+                                                   result.keys_.data(), result.distances_.data(), &error);
+            if (error) return result.failed(error);
+            return result;
+        }
+        std::vector<vector_key_t> live(size()), allowed;
+        live.resize(usearch_b200_export_keys(handle_, 0, live.size(), live.data(), &error));
+        if (error) return result.failed(error);
+        for (vector_key_t key : live)
+            if (predicate(key)) allowed.push_back(key);
+        std::uint64_t const offsets[2] = {0, allowed.size()};
+        std::size_t count = 0;
+        std::uint64_t computed = 0;
+        usearch_b200_grouped_filtered_exact_search_many(handle_, vector, 1, 0, scalar_kind<scalar_at>(), wanted, nullptr, offsets, 1,
+                                                        allowed.data(), result.keys_.data(), result.distances_.data(), &count, &computed,
+                                                        &error);
+        if (error) return result.failed(error);
+        result.count = count;
+        result.computed_distances = computed;
+        return result;
+    }
     /* index_dense.hpp:1595-1608, the live keys in slot order */
     void export_keys(vector_key_t* keys, std::size_t offset, std::size_t limit) const {
         usearch_b200_export_keys(handle_, offset, limit, keys, nullptr);

@@ -179,10 +179,11 @@ usearch_index_t usearch_init(usearch_init_options_t* options, usearch_error_t* e
 
 void usearch_free(usearch_index_t index, usearch_error_t*) { delete as_index(index); }
 
-size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table and the grouped filter's
-                                                                        bitmap rows count once they exist */
+size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table, the grouped filter's bitmap
+                                                                        rows and the exact filter's scratch count once they exist */
     frozen_index_t const* ix = as_index(index);
-    return ix->hbm_bytes + ix->key_table.cells.capacity * sizeof(key_cell_t) + ix->group_bits.capacity * sizeof(uint32_t);
+    return ix->hbm_bytes + ix->key_table.cells.capacity * sizeof(key_cell_t) + ix->group_bits.capacity * sizeof(uint32_t) +
+           ix->exact_filter.bytes();
 }
 
 char const* usearch_hardware_acceleration(usearch_index_t, usearch_error_t*) { return "sm_90a"; }
@@ -446,6 +447,44 @@ void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, voi
         return ix->grouped_filtered_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
                                                   keys, distances, counts, computed_distances, visited_members,
                                                   cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
+    }));
+}
+
+/* exact filtered search (grouped_filter.cu): search_exact_ over only the live slots of each query's key set */
+size_t usearch_b200_grouped_filtered_exact_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                       size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                       uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                       usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                       size_t* counts, uint64_t* computed_distances, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    uint32_t qs = scalar_to_char(query_kind);
+    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
+    std::vector<size_t> own(counts ? 0 : queries_count);
+    size_t* const found = counts ? counts : own.data();
+    if (char const* e = guarded([&] {
+            return ix->grouped_exact_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count, set_keys, keys,
+                                                 distances, found, computed_distances);
+        })) {
+        set_error(error, e);
+        return 0;
+    }
+    size_t total = 0;
+    for (size_t i = 0; i < queries_count && count; ++i) total += found[i];
+    return total;
+}
+
+void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                            size_t queries_stride, size_t count, uint32_t const* groups,
+                                                            uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                            usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                            uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        return ix->grouped_exact_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys, keys,
+                                               distances, counts, computed_distances, nullptr,
+                                               cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
     }));
 }
 

@@ -5,10 +5,16 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <type_traits>
 
 #include "device_index.h"
 
 namespace usearch_b200 {
+
+/* one CTA row of a listed launch: `count` queries from `first` (sorted by set) against one set's ascending slot list */
+struct exact_item_t {
+    uint32_t first, count, list_begin, list_len;
+};
 
 struct exact_args_t {
     uint8_t const* queries = nullptr; /* rows padded to vec_stride, index scalar kind */
@@ -28,12 +34,35 @@ struct exact_args_t {
     int const* vector_norms = nullptr;
 };
 
+/* the LISTED kernels' arguments (exact filtered search): the fields above, then the lists. CTA x serves items[x], whose
+ * queries are `first ..` of the gathered batch and whose rows are slots rows[list_begin ..]; each list is cut into
+ * `segments` runs of ceil(len / segments) rounded up to the tile, and vector_norms is indexed by list position. The
+ * kernels that serve every slot, and the merge, keep exact_args_t itself. */
+struct exact_listed_args_t : exact_args_t {
+    exact_item_t const* items = nullptr;
+    uint32_t const* rows = nullptr;
+};
+template <bool LISTED> using exact_args_of = typename std::conditional<LISTED, exact_listed_args_t, exact_args_t>::type;
+
+/* positions [lo, hi) of segment `seg` of a listed item, segments a multiple of `tile` long */
+__device__ __forceinline__ void listed_segment(exact_item_t const& it, uint32_t segments, uint32_t seg, uint32_t tile, uint32_t& lo,
+                                               uint32_t& hi) {
+    uint32_t len = (it.list_len + segments - 1) / segments;
+    len = (len + tile - 1) / tile * tile;
+    lo = min(it.list_len, seg * len);
+    hi = min(it.list_len, lo + len);
+}
+
 /* exact_imma.cu: i8 on the tensor cores */
 size_t exact_imma_smem_bytes();
 int exact_imma_tile_queries();
 int exact_imma_tile_vectors();
 cudaError_t exact_imma_self_dots(uint8_t const* rows, uint64_t stride, uint32_t chunks16, uint32_t count, int* out, cudaStream_t stream);
 cudaError_t exact_imma_launch(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, cudaStream_t stream);
+/* listed (exact filtered) twins: b2 of slots rows[0 .. count) by list position, and the LISTED kernel (metric(query, stored)) */
+cudaError_t exact_imma_listed_self_dots(uint8_t const* vectors, uint64_t stride, uint32_t chunks16, uint32_t const* rows, uint32_t count,
+                                        int* out, cudaStream_t stream);
+cudaError_t exact_imma_listed_launch(device_index_t const& ix, exact_listed_args_t const& a, dim3 grid, cudaStream_t stream);
 
 /* exact_wgmma.cu: the same scan on warpgroup MMAs (wgmma, TMA operand loads) */
 size_t exact_wgmma_smem_bytes();

@@ -69,15 +69,44 @@ __global__ void i8_self_dot_kernel(uint8_t const* rows, uint64_t stride, uint32_
     if (lane == 0) out[row] = s;
 }
 
-template <uint32_t METRIC, bool SWAP>
+/* sum of squares of the listed rows: out[j] for slot rows[j] (listed scans index the stored norms by list position) */
+__global__ void i8_listed_self_dot_kernel(uint8_t const* vectors, uint64_t stride, uint32_t chunks16, uint32_t const* rows, uint32_t count,
+                                          int* out) {
+    uint32_t const j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    int const lane = threadIdx.x & 31;
+    if (j >= count) return;
+    uint4 const* v4 = reinterpret_cast<uint4 const*>(vectors + (size_t)rows[j] * stride);
+    int s = 0;
+    for (uint32_t c = lane; c < chunks16; c += 32) {
+        uint4 const x = v4[c];
+        s = __dp4a((int)x.x, (int)x.x, s); s = __dp4a((int)x.y, (int)x.y, s);
+        s = __dp4a((int)x.z, (int)x.z, s); s = __dp4a((int)x.w, (int)x.w, s);
+    }
+    s = reduce_add_i32<32>(s);
+    if (lane == 0) out[j] = s;
+}
+
+/* LISTED: the CTA serves work item a.items[blockIdx.x]; column j of its segment is slot a.rows[list_begin + j] and its
+ * b2 is a.vector_norms[list_begin + j] (exact_args.h) */
+template <uint32_t METRIC, bool SWAP, bool LISTED = false>
 __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_constant__ device_index_t const ix,
-                                                                   __grid_constant__ exact_args_t const a) {
+                                                                   __grid_constant__ exact_args_of<LISTED> const a) {
     extern __shared__ __align__(128) uint8_t smem[];
     int const tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
     int const wm = warp >> 2, wn = warp & 3; /* warp tile: rows wm*64.., columns wn*32.. */
     uint32_t const vs = (uint32_t)ix.vec_stride, nks = (vs + IM_BK - 1) / IM_BK;
-    uint32_t const q0 = blockIdx.x * IM_BM;
-    uint32_t const seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
+    uint32_t q0 = blockIdx.x * IM_BM, q_end = 0; /* LISTED: queries from q_end on are dead rows */
+    uint32_t seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
+    uint32_t const* listed_slots = nullptr;
+    int const* vnorms = nullptr;
+    if constexpr (LISTED) {
+        exact_item_t const it = a.items[blockIdx.x];
+        q0 = it.first;
+        q_end = it.first + it.count;
+        listed_segment(it, a.segments, blockIdx.y, IM_BN, seg_lo, seg_hi);
+        listed_slots = a.rows + it.list_begin;
+        vnorms = a.vector_norms + it.list_begin;
+    }
     uint32_t const ntiles = seg_hi > seg_lo ? (seg_hi - seg_lo + IM_BN - 1) / IM_BN : 0;
 
     float* const dist = reinterpret_cast<float*>(smem); /* aliases the pipeline, used between K loops only */
@@ -91,7 +120,7 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
     uint32_t const pipe = smem_u32(smem);
 
     if (tid < IM_BM) {
-        qa2[tid] = (METRIC != METRIC_IP && q0 + tid < a.nq) ? a.query_norms[q0 + tid] : 0;
+        qa2[tid] = (METRIC != METRIC_IP && q0 + tid < (LISTED ? q_end : a.nq)) ? a.query_norms[q0 + tid] : 0;
         qrn[tid] = METRIC == METRIC_COS ? i8_rnorm(qa2[tid]) : 0.f;
         rsize[tid] = 0;
         rworst[tid] = 0.f;
@@ -102,7 +131,7 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
 #pragma unroll
         for (int i = 0; i < 2; ++i) { /* 512 chunks of the query part */
             uint32_t const c = (uint32_t)tid + (uint32_t)i * IM_THREADS, row = c >> 2, off = (c & 3u) * 16u;
-            bool const ok = q0 + row < a.nq && kbyte + off < vs;
+            bool const ok = q0 + row < (LISTED ? q_end : a.nq) && kbyte + off < vs;
             void const* src = ok ? a.queries + (size_t)(q0 + row) * a.query_stride + kbyte + off : a.queries;
             cp_async16(sbase + row * IM_BK + off, src, ok);
         }
@@ -110,7 +139,8 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
         for (int i = 0; i < 2; ++i) { /* 512 chunks of the stored part */
             uint32_t const c = (uint32_t)tid + (uint32_t)i * IM_THREADS, row = c >> 2, off = (c & 3u) * 16u;
             bool const ok = tile_base + row < seg_hi && kbyte + off < vs;
-            void const* src = ok ? ix.vectors + (size_t)(tile_base + row) * ix.vec_stride + kbyte + off : ix.vectors;
+            void const* src = ok ? ix.vectors + (size_t)(LISTED ? listed_slots[tile_base + row] : tile_base + row) * ix.vec_stride + kbyte + off
+                                 : ix.vectors;
             cp_async16(sbase + IM_BM * IM_BK + row * IM_BK + off, src, ok);
         }
     };
@@ -124,10 +154,11 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
             cp_async_commit();
         }
         if (tid < IM_BN) { /* per-column facts of this tile */
-            uint32_t const slot = tile_base + (uint32_t)tid;
-            bool usable = slot < seg_hi;
+            uint32_t const pos = tile_base + (uint32_t)tid;
+            uint32_t const slot = LISTED ? (pos < seg_hi ? listed_slots[pos] : 0u) : pos;
+            bool usable = pos < seg_hi;
             if (usable && ix.deleted_bits) usable = !((ix.deleted_bits[slot >> 5] >> (slot & 31)) & 1u);
-            vb2[tid] = (METRIC != METRIC_IP && slot < seg_hi) ? a.vector_norms[slot] : 0;
+            vb2[tid] = (METRIC != METRIC_IP && pos < seg_hi) ? (LISTED ? vnorms : a.vector_norms)[pos] : 0;
             vrn[tid] = METRIC == METRIC_COS ? i8_rnorm(vb2[tid]) : 0.f;
             uint32_t const m = __ballot_sync(0xffffffffu, usable);
             if (lane == 0) vmask[warp] = m;
@@ -190,7 +221,7 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
         for (int rr = 0; rr < 16; ++rr) {
             int const row = warp * 16 + rr;
             uint32_t const qi = q0 + (uint32_t)row;
-            if (qi >= a.nq) break; /* warp-uniform */
+            if (qi >= (LISTED ? q_end : a.nq)) break; /* warp-uniform */
             uint32_t size = rsize[row];
             float worst = rworst[row];
             size_t const list = ((size_t)qi * a.segments + blockIdx.y) * a.k;
@@ -210,7 +241,8 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
                         int const src_lane = __ffs(todo) - 1;
                         todo &= todo - 1;
                         float const cd = __shfl_sync(0xffffffffu, dv[c], src_lane);
-                        uint32_t const cs = tile_base + (uint32_t)(src_lane * 4 + c);
+                        uint32_t cs = tile_base + (uint32_t)(src_lane * 4 + c);
+                        if constexpr (LISTED) cs = listed_slots[cs];
                         if (size < a.k || !(cd > worst)) {
                             top_insert_global_keyed(a.part_d + list, a.part_s + list, size, a.k, cd, cs, lane);
                             if (size == a.k) worst = reinterpret_cast<float volatile*>(a.part_d)[list + a.k - 1];
@@ -223,7 +255,7 @@ __global__ void __launch_bounds__(IM_THREADS, 2) exact_imma_kernel(__grid_consta
         __syncthreads(); /* the distance tile is free again: the next prologue may refill the stages */
     }
 
-    if (tid < IM_BM && q0 + tid < a.nq) a.part_n[(size_t)(q0 + tid) * a.segments + blockIdx.y] = rsize[tid];
+    if (tid < IM_BM && q0 + tid < (LISTED ? q_end : a.nq)) a.part_n[(size_t)(q0 + tid) * a.segments + blockIdx.y] = rsize[tid];
 }
 
 size_t exact_imma_smem_bytes() { return IM_PIPE_BYTES + (IM_BM + IM_BN) * 8 + IM_BM * 8 + 16; }
@@ -233,6 +265,14 @@ int exact_imma_tile_vectors() { return IM_BN; }
 cudaError_t exact_imma_self_dots(uint8_t const* rows, uint64_t stride, uint32_t chunks16, uint32_t count, int* out, cudaStream_t stream) {
     if (!count) return cudaSuccess;
     i8_self_dot_kernel<<<(count * 32u + 255u) / 256u, 256, 0, stream>>>(rows, stride, chunks16, count, out);
+    return cudaGetLastError();
+}
+
+cudaError_t exact_imma_listed_self_dots(uint8_t const* vectors, uint64_t stride, uint32_t chunks16, uint32_t const* rows, uint32_t count,
+                                        int* out, cudaStream_t stream) {
+    if (!count) return cudaSuccess;
+    i8_listed_self_dot_kernel<<<(unsigned)(((uint64_t)count * 32u + 255u) / 256u), 256, 0, stream>>>(vectors, stride, chunks16, rows, count,
+                                                                                                      out);
     return cudaGetLastError();
 }
 
@@ -248,6 +288,24 @@ template <uint32_t METRIC> static cudaError_t imma_launch_t(device_index_t const
         exact_imma_kernel<METRIC, false><<<grid, IM_THREADS, smem, stream>>>(ix, a);
     }
     return cudaGetLastError();
+}
+
+template <uint32_t METRIC> static cudaError_t imma_listed_launch_t(exact_listed_args_t const& a, device_index_t const& ix, dim3 grid,
+                                                                 cudaStream_t stream) {
+    size_t const smem = exact_imma_smem_bytes();
+    cudaError_t e = cudaFuncSetAttribute(exact_imma_kernel<METRIC, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    exact_imma_kernel<METRIC, false, true><<<grid, IM_THREADS, smem, stream>>>(ix, a);
+    return cudaGetLastError();
+}
+
+cudaError_t exact_imma_listed_launch(device_index_t const& ix, exact_listed_args_t const& a, dim3 grid, cudaStream_t stream) {
+    switch (ix.metric) {
+    case METRIC_IP: return imma_listed_launch_t<METRIC_IP>(a, ix, grid, stream);
+    case METRIC_L2SQ: return imma_listed_launch_t<METRIC_L2SQ>(a, ix, grid, stream);
+    case METRIC_COS: return imma_listed_launch_t<METRIC_COS>(a, ix, grid, stream);
+    default: return cudaErrorInvalidValue;
+    }
 }
 
 cudaError_t exact_imma_launch(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, cudaStream_t stream) {

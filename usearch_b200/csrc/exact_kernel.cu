@@ -72,18 +72,27 @@ template <bool STAGED> __device__ __forceinline__ uint4 scan_chunk(uint4 const* 
 
 /* STAGED = false: the query and the rows are read from global memory where they lie, for rows too long to stage 8 queries
  * and 2 x VPP rows in 227 KB. Each lane group walks the same chunks in the same order through the same metric calls,
- * so both variants give the same bits. */
-template <class M, bool SWAP, bool STAGED>
+ * so both variants give the same bits.
+ * LISTED: the CTA serves work item a.items[blockIdx.x]; row j of its segment is slot a.rows[list_begin + j] (exact_args.h). */
+template <class M, bool SWAP, bool STAGED, bool LISTED = false>
 __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_constant__ device_index_t const ix,
-                                                                      __grid_constant__ exact_args_t const a) {
+                                                                      __grid_constant__ exact_args_of<LISTED> const a) {
     constexpr int LPV = M::LPV, VPP = 32 / LPV;
     extern __shared__ __align__(128) uint8_t smem[];
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane / LPV, sub = lane % LPV;
     uint32_t const chunks = ix.chunks16, bytes = (uint32_t)ix.vec_stride;
     uint32_t const bars = smem_u32(smem + a.off_bars), stage_addr = smem_u32(smem + a.off_stage);
-    uint32_t const qi = blockIdx.x * EXACT_WARPS + warp;
-    bool const has_query = qi < a.nq;
-    uint32_t const seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
+    uint32_t qi = blockIdx.x * EXACT_WARPS + warp;
+    bool has_query = qi < a.nq;
+    uint32_t seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
+    uint32_t const* list = nullptr; /* LISTED: the slots of this item's rows */
+    if constexpr (LISTED) {
+        exact_item_t const it = a.items[blockIdx.x];
+        qi = it.first + (uint32_t)warp;
+        has_query = (uint32_t)warp < it.count;
+        listed_segment(it, a.segments, blockIdx.y, VPP, seg_lo, seg_hi);
+        list = a.rows + it.list_begin;
+    }
     uint32_t const ntiles = seg_hi > seg_lo ? (seg_hi - seg_lo + VPP - 1) / VPP : 0;
     uint4 const* q4; /* a dead query slot reads query 0: prepare() shuffles across the whole warp */
     if constexpr (STAGED) {
@@ -111,8 +120,8 @@ __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_con
         uint32_t const base = seg_lo + t * VPP, cnt = min((uint32_t)VPP, seg_hi - base), set = t & 1u;
         mbar_expect_tx(bars + 8u * set, cnt * bytes);
         for (uint32_t i = 0; i < cnt; ++i)
-            bulk_copy_g2s(stage_addr + (set * VPP + i) * a.stage_stride, ix.vectors + (size_t)(base + i) * ix.vec_stride, bytes,
-                          bars + 8u * set);
+            bulk_copy_g2s(stage_addr + (set * VPP + i) * a.stage_stride,
+                          ix.vectors + (size_t)(LISTED ? list[base + i] : base + i) * ix.vec_stride, bytes, bars + 8u * set);
     };
     if constexpr (STAGED)
         if (threadIdx.x == 0 && ntiles) issue(0);
@@ -131,8 +140,9 @@ __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_con
             mbar_wait(bars + 8u * set, (phase >> set) & 1u);
             phase ^= 1u << set;
         }
-        uint32_t const slot = base + (uint32_t)g;
         bool const act = has_query && (uint32_t)g < cnt;
+        uint32_t slot = base + (uint32_t)g;
+        if constexpr (LISTED) slot = act ? list[slot] : 0u;
         typename M::acc_t acc;
         M::init(acc);
         if (act) {
@@ -166,7 +176,7 @@ __global__ void __launch_bounds__(EXACT_WARPS * 32) exact_scan_kernel(__grid_con
             int const src_lane = __ffs(todo) - 1;
             todo &= todo - 1;
             float const cd = __shfl_sync(0xffffffffu, d, src_lane);
-            uint32_t const cs = base + (uint32_t)(src_lane / LPV);
+            uint32_t const cs = LISTED ? __shfl_sync(0xffffffffu, slot, src_lane) : base + (uint32_t)(src_lane / LPV);
             if (top_size < a.k || !(cd > worst)) {
                 top_insert_reg_keyed(td, ts, top_size, a.k, cd, cs, lane);
                 worst = top_back_reg(td, top_size);
@@ -197,17 +207,26 @@ template <class M> struct exact_tile_t {
     static constexpr int QPC = TILED_WARPS * QT;    /* queries per CTA */
 };
 
-template <class M, bool SWAP>
+template <class M, bool SWAP, bool LISTED = false>
 __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid_constant__ device_index_t const ix,
-                                                                          __grid_constant__ exact_args_t const a) {
+                                                                          __grid_constant__ exact_args_of<LISTED> const a) {
     using T = exact_tile_t<M>;
     constexpr int LPV = M::LPV, QT = T::QT, VT = T::VT, TV = T::TV, GROUPS = 32 / LPV;
     extern __shared__ __align__(128) uint8_t smem[];
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane / LPV, sub = lane % LPV;
     uint32_t const chunks = ix.chunks16, bytes = (uint32_t)ix.vec_stride;
     uint32_t const bars = smem_u32(smem + a.off_bars), stage_addr = smem_u32(smem + a.off_stage);
-    uint32_t const q0 = blockIdx.x * T::QPC + (uint32_t)warp * QT; /* first query of this warp */
-    uint32_t const seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
+    uint32_t q0 = blockIdx.x * T::QPC + (uint32_t)warp * QT; /* first query of this warp */
+    uint32_t q_end = 0;                                         /* LISTED: queries from q_end on are dead slots */
+    uint32_t seg_lo = blockIdx.y * a.segment_len, seg_hi = min(ix.n, seg_lo + a.segment_len);
+    uint32_t const* list = nullptr;
+    if constexpr (LISTED) {
+        exact_item_t const it = a.items[blockIdx.x];
+        q0 = it.first + (uint32_t)warp * QT;
+        q_end = it.first + it.count;
+        listed_segment(it, a.segments, blockIdx.y, TV, seg_lo, seg_hi);
+        list = a.rows + it.list_begin;
+    }
     uint32_t const ntiles = seg_hi > seg_lo ? (seg_hi - seg_lo + TV - 1) / TV : 0;
 
     if (threadIdx.x == 0) {
@@ -221,7 +240,7 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
     for (int qi = 0; qi < QT; ++qi) {
         uint4* dst = reinterpret_cast<uint4*>(smem + a.off_queries + (size_t)(warp * QT + qi) * bytes);
         qrow[qi] = dst;
-        bool const live = q0 + qi < a.nq;
+        bool const live = q0 + qi < (LISTED ? q_end : a.nq);
         uint4 const* src = reinterpret_cast<uint4 const*>(a.queries + (size_t)(live ? q0 + qi : 0) * a.query_stride);
         for (uint32_t j = lane; j < chunks; j += 32) dst[j] = live ? src[j] : make_uint4(0u, 0u, 0u, 0u);
     }
@@ -241,8 +260,8 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
         if (lane == 0) mbar_expect_tx(bars + 8u * set, cnt * bytes);
         __syncwarp();
         for (uint32_t i = lane; i < cnt; i += 32)
-            bulk_copy_g2s(stage_addr + (set * TV + i) * a.stage_stride, ix.vectors + (size_t)(base + i) * ix.vec_stride, bytes,
-                          bars + 8u * set);
+            bulk_copy_g2s(stage_addr + (set * TV + i) * a.stage_stride,
+                          ix.vectors + (size_t)(LISTED ? list[base + i] : base + i) * ix.vec_stride, bytes, bars + 8u * set);
     };
     if (warp == 0 && ntiles) issue(0);
 
@@ -282,7 +301,8 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
 
 #pragma unroll
         for (int vt = 0; vt < VT; ++vt) {
-            uint32_t const in_tile = (uint32_t)(vt * GROUPS + g), slot = base + in_tile;
+            uint32_t const in_tile = (uint32_t)(vt * GROUPS + g),
+                           slot = LISTED ? (in_tile < cnt ? list[base + in_tile] : 0u) : base + in_tile;
             bool usable = in_tile < cnt;
             float b2 = 0.f;
             if constexpr (M::NORMS) b2 = usable ? __ldg(ix.norms + slot) : 0.f;
@@ -294,7 +314,7 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
                 float d = finish_ordered<M, SWAP>(acc[qi][vt], qc[qi]);
                 if constexpr (M::NORMS)
                     d = SWAP ? M::finalize_rn(d, b2, qc[qi].a2, v_rn, q_rn[qi]) : M::finalize_rn(d, qc[qi].a2, b2, q_rn[qi], v_rn);
-                bool const live = q0 + qi < a.nq;
+                bool const live = q0 + qi < (LISTED ? q_end : a.nq);
                 uint32_t todo = __ballot_sync(0xffffffffu, usable && live && (sizes[qi] < a.k || !(d > worst[qi])));
                 if (todo) {
                     size_t const row = ((size_t)(q0 + qi) * a.segments + blockIdx.y) * a.k;
@@ -302,7 +322,7 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
                         int const src_lane = __ffs(todo) - 1;
                         todo &= todo - 1;
                         float const cd = __shfl_sync(0xffffffffu, d, src_lane);
-                        uint32_t const cs = base + (uint32_t)(vt * GROUPS + src_lane / LPV);
+                        uint32_t const cs = LISTED ? __shfl_sync(0xffffffffu, slot, src_lane) : base + (uint32_t)(vt * GROUPS + src_lane / LPV);
                         if (sizes[qi] < a.k || !(cd > worst[qi])) {
                             top_insert_global_keyed(a.part_d + row, a.part_s + row, sizes[qi], a.k, cd, cs, lane);
                             if (sizes[qi] == a.k) worst[qi] = reinterpret_cast<float volatile*>(a.part_d)[row + a.k - 1];
@@ -317,7 +337,7 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
     if (lane == 0) {
 #pragma unroll
         for (int qi = 0; qi < QT; ++qi)
-            if (q0 + qi < a.nq) a.part_n[(size_t)(q0 + qi) * a.segments + blockIdx.y] = sizes[qi];
+            if (q0 + qi < (LISTED ? q_end : a.nq)) a.part_n[(size_t)(q0 + qi) * a.segments + blockIdx.y] = sizes[qi];
     }
 }
 
@@ -387,9 +407,13 @@ __global__ void exact_merge_big_kernel(device_index_t ix, exact_args_t a, float*
     if (lane == 0) a.out_counts[qi] = top_size;
 }
 
-template <class M, bool STAGED> static cudaError_t exact_launch_scan_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid,
-                                                                      size_t smem, cudaStream_t stream) {
-    if (swap) {
+template <class M, bool STAGED> static cudaError_t exact_launch_scan_t(device_index_t const& ix, exact_listed_args_t const& a, bool swap, bool listed,
+                                                                      dim3 grid, size_t smem, cudaStream_t stream) {
+    if (listed) { /* index mode only: metric(query, stored) */
+        cudaError_t e = cudaFuncSetAttribute(exact_scan_kernel<M, false, STAGED, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        exact_scan_kernel<M, false, STAGED, true><<<grid, EXACT_WARPS * 32, smem, stream>>>(ix, a);
+    } else if (swap) {
         cudaError_t e = cudaFuncSetAttribute(exact_scan_kernel<M, true, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         exact_scan_kernel<M, true, STAGED><<<grid, EXACT_WARPS * 32, smem, stream>>>(ix, a);
@@ -402,14 +426,19 @@ template <class M, bool STAGED> static cudaError_t exact_launch_scan_t(device_in
 }
 
 /* smem == 0: the staged scan does not fit, rows are read in place */
-template <class M> static cudaError_t exact_launch_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, size_t smem,
-                                                     cudaStream_t stream) {
-    return smem ? exact_launch_scan_t<M, true>(ix, a, swap, grid, smem, stream) : exact_launch_scan_t<M, false>(ix, a, swap, grid, 0, stream);
+template <class M> static cudaError_t exact_launch_t(device_index_t const& ix, exact_listed_args_t const& a, bool swap, bool listed, dim3 grid,
+                                                     size_t smem, cudaStream_t stream) {
+    return smem ? exact_launch_scan_t<M, true>(ix, a, swap, listed, grid, smem, stream)
+                : exact_launch_scan_t<M, false>(ix, a, swap, listed, grid, 0, stream);
 }
 
-template <class M> static cudaError_t exact_launch_tiled_t(device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid, size_t smem,
-                                                           cudaStream_t stream) {
-    if (swap) {
+template <class M> static cudaError_t exact_launch_tiled_t(device_index_t const& ix, exact_listed_args_t const& a, bool swap, bool listed, dim3 grid,
+                                                           size_t smem, cudaStream_t stream) {
+    if (listed) {
+        cudaError_t e = cudaFuncSetAttribute(exact_tiled_kernel<M, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        exact_tiled_kernel<M, false, true><<<grid, TILED_WARPS * 32, smem, stream>>>(ix, a);
+    } else if (swap) {
         cudaError_t e = cudaFuncSetAttribute(exact_tiled_kernel<M, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         exact_tiled_kernel<M, true><<<grid, TILED_WARPS * 32, smem, stream>>>(ix, a);
@@ -421,9 +450,9 @@ template <class M> static cudaError_t exact_launch_tiled_t(device_index_t const&
     return cudaGetLastError();
 }
 
-template <class M> static cudaError_t exact_launch_any_t(bool tiled, device_index_t const& ix, exact_args_t const& a, bool swap, dim3 grid,
-                                                         size_t smem, cudaStream_t stream) {
-    return tiled ? exact_launch_tiled_t<M>(ix, a, swap, grid, smem, stream) : exact_launch_t<M>(ix, a, swap, grid, smem, stream);
+template <class M> static cudaError_t exact_launch_any_t(bool tiled, device_index_t const& ix, exact_listed_args_t const& a, bool swap, bool listed,
+                                                         dim3 grid, size_t smem, cudaStream_t stream) {
+    return tiled ? exact_launch_tiled_t<M>(ix, a, swap, listed, grid, smem, stream) : exact_launch_t<M>(ix, a, swap, listed, grid, smem, stream);
 }
 
 static int exact_lpv(device_index_t const& ix) {
@@ -436,10 +465,12 @@ static int exact_lpv(device_index_t const& ix) {
  *  Exact top-k of `nq` device-resident queries (index scalar kind, rows `query_stride` bytes apart, 16-byte aligned
  *  and readable up to vec_stride) against every vector of `ix`. `swap` = call the metric as metric(stored, query).
  *  Scratch for the per-segment partial lists is taken from `scratch` (grown on demand).
+ *  `listed` (exact filtered search, swap = false): the CTAs serve its work items against their slot lists instead; with
+ *  `listed->items == nullptr` nothing runs and `listed->qpc` receives the queries per item of the kernel that would.
  */
-char const* exact_search_device(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t query_stride, size_t k,
-                                bool swap, bool slots_as_keys, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
-                                device_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
+static char const* exact_run(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t query_stride, size_t k,
+                             bool swap, bool slots_as_keys, exact_listed_t* listed, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                             device_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
     if (!nq || !k) return nullptr;
     /* count <= 256: k-best lists in registers (scan, IMMA, merge); beyond that the tiled kernel's global-memory lists and
      * exact_merge_big_kernel carry any count (search_exact_ takes any `wanted`, index.hpp:4251-4268) */
@@ -451,7 +482,7 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
         return nullptr;
     }
     int const lpv = exact_lpv(ix);
-    exact_args_t a;
+    exact_listed_args_t a; /* the listed fields stay null for a scan of every slot */
     a.queries = static_cast<uint8_t const*>(d_queries);
     a.query_stride = query_stride;
     a.nq = (uint32_t)nq;
@@ -469,8 +500,9 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     bool const imma = !big_k && ix.scalar == SCALAR_I8 && (forced == 0 || forced == 3 || forced == 4) &&
                       (ix.metric == METRIC_IP || ix.metric == METRIC_L2SQ || ix.metric == METRIC_COS);
     if ((forced == 3 || forced == 4) && !imma) return "The tensor-core exact-search kernels serve i8 vectors only";
-    /* wgmma (exact_wgmma.cu) when the driver can encode tensor maps; mma.sync (exact_imma.cu) otherwise or when forced */
-    bool const wgmma = imma && forced != 3 && exact_wgmma_usable(ix, a); /* count <= 24; larger counts stay on mma.sync */
+    /* wgmma (exact_wgmma.cu) when the driver can encode tensor maps; mma.sync (exact_imma.cu) otherwise or when forced.
+     * Its TMA tensor maps read contiguous slabs and cannot follow a slot list: listed scans take mma.sync. */
+    bool const wgmma = !listed && imma && forced != 3 && exact_wgmma_usable(ix, a); /* count <= 24; larger counts stay on mma.sync */
     bool const tiled = !imma && (forced == 1 && !big_k ? false : tiled_smem <= 227 * 1024);
     if (big_k && !tiled) return "Exact search with count > 256 needs vectors that fit the tiled stage";
     if (forced == 2 && !tiled) return "Vectors too long for the tiled exact-search stage";
@@ -486,11 +518,18 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     /* only the one-query-per-warp scan can outgrow its stage (the tiled one is not chosen then): it reads in place */
     bool const in_place = smem > 227 * 1024;
     if (in_place) smem = 0;
-    uint32_t const groups = (uint32_t)((nq + qpc - 1) / qpc);
+    if (listed && !listed->items) {
+        listed->qpc = qpc;
+        return nullptr;
+    }
+    bool const is_listed = listed != nullptr;
+    uint32_t const groups = is_listed ? listed->n_items : (uint32_t)((nq + qpc - 1) / qpc);
+    uint32_t const scanned = is_listed ? listed->total_rows : ix.n; /* rows the segments share out */
     /* cut the dataset so that the grid fills whole waves of the resident CTAs (1 per SM tiled, ~3 per SM staged, 4 per SM
      * in place: up to 64 registers) */
     uint32_t const resident = (uint32_t)sm_count * (wgmma ? 1u : (imma ? 2u : (tiled ? 1u : (in_place ? 4u : 3u))));
-    uint32_t const max_segments = std::max<uint32_t>(1, std::min<uint32_t>((ix.n + 8 * (uint32_t)vpp - 1) / (8 * (uint32_t)vpp), 65535u));
+    uint32_t const max_segments =
+        std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(((uint64_t)scanned + 8 * (uint32_t)vpp - 1) / (8 * (uint32_t)vpp)), 65535u));
     uint32_t segments = 1;
     {
         double best = -1;
@@ -504,15 +543,22 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     }
     size_t const list_bytes = nq * k * 8;
     while (segments > 1 && list_bytes * segments > ((size_t)1 << 30)) --segments;
-    uint32_t seg_len = (ix.n + segments - 1) / segments;
-    seg_len = (seg_len + (uint32_t)vpp - 1) / (uint32_t)vpp * (uint32_t)vpp;
-    segments = (ix.n + seg_len - 1) / seg_len;
-    a.segments = segments;
-    a.segment_len = seg_len;
+    if (is_listed) { /* every item cuts its own list into `segments` (listed_segment); some may come out empty */
+        a.segments = segments;
+        a.segment_len = 0;
+        a.items = listed->items;
+        a.rows = listed->rows;
+    } else {
+        uint32_t seg_len = (ix.n + segments - 1) / segments;
+        seg_len = (seg_len + (uint32_t)vpp - 1) / (uint32_t)vpp * (uint32_t)vpp;
+        segments = (ix.n + seg_len - 1) / seg_len;
+        a.segments = segments;
+        a.segment_len = seg_len;
+    }
     size_t const rows = nq * segments;
     size_t const lists = rows * k * 8 + rows * 4;
     size_t const norms_at = (lists + 15) / 16 * 16;
-    size_t const need = norms_at + (imma ? (nq + (size_t)ix.n) * 4 : 0) + (big_k ? nq * k * 8 : 0) + 64;
+    size_t const need = norms_at + (imma ? (nq + (size_t)scanned) * 4 : 0) + (big_k ? nq * k * 8 : 0) + 64;
     if (char const* e = scratch.reserve(need)) return e;
     a.part_d = reinterpret_cast<float*>(scratch.ptr);
     a.part_s = reinterpret_cast<uint32_t*>(scratch.ptr + rows * k * 4);
@@ -520,8 +566,9 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     if (imma && ix.metric != METRIC_IP) {
         int* qn = reinterpret_cast<int*>(scratch.ptr + norms_at);
         int* vn = qn + nq;
-        if (exact_imma_self_dots(a.queries, query_stride, ix.chunks16, (uint32_t)nq, qn, stream) != cudaSuccess ||
-            exact_imma_self_dots(ix.vectors, ix.vec_stride, ix.chunks16, ix.n, vn, stream) != cudaSuccess)
+        cudaError_t const ev = is_listed ? exact_imma_listed_self_dots(ix.vectors, ix.vec_stride, ix.chunks16, listed->rows, scanned, vn, stream)
+                                         : exact_imma_self_dots(ix.vectors, ix.vec_stride, ix.chunks16, ix.n, vn, stream);
+        if (exact_imma_self_dots(a.queries, query_stride, ix.chunks16, (uint32_t)nq, qn, stream) != cudaSuccess || ev != cudaSuccess)
             return "CUDA failure: i8 norms launch";
         a.query_norms = qn;
         a.vector_norms = vn;
@@ -532,37 +579,37 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
     dim3 const grid(groups, segments);
     cudaError_t e = cudaErrorInvalidValue;
     if (wgmma) e = exact_wgmma_launch(ix, a, swap, grid, stream);
-    else if (imma) e = exact_imma_launch(ix, a, swap, grid, stream);
+    else if (imma) e = is_listed ? exact_imma_listed_launch(ix, a, grid, stream) : exact_imma_launch(ix, a, swap, grid, stream);
     else switch (ix.scalar) {
     case SCALAR_F32:
-        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_f32_t>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_f32_t>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_f32_t>(tiled, ix, a, swap, grid, smem, stream);
+        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_f32_t>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_f32_t>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_f32_t>(tiled, ix, a, swap, is_listed, grid, smem, stream);
         break;
     case SCALAR_F64:
-        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_f64_t>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_f64_t>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_f64_t>(tiled, ix, a, swap, grid, smem, stream);
+        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_f64_t>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_f64_t>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_f64_t>(tiled, ix, a, swap, is_listed, grid, smem, stream);
         break;
     case SCALAR_F16:
-        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_half_t<f16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_half_t<f16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_half_t<f16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
+        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_half_t<f16_conv_t>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_half_t<f16_conv_t>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_half_t<f16_conv_t>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
         break;
     case SCALAR_BF16:
-        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_half_t<bf16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_half_t<bf16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_half_t<bf16_conv_t>>(tiled, ix, a, swap, grid, smem, stream);
+        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_half_t<bf16_conv_t>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_half_t<bf16_conv_t>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_half_t<bf16_conv_t>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
         break;
     case SCALAR_I8:
-        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_i8_t<4>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_i8_t<4>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_i8_t<4>>(tiled, ix, a, swap, grid, smem, stream);
+        if (ix.metric == METRIC_L2SQ) e = exact_launch_any_t<l2sq_i8_t<4>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_IP) e = exact_launch_any_t<ip_i8_t<4>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_COS) e = exact_launch_any_t<cos_i8_t<4>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
         break;
     case SCALAR_B1:
-        if (ix.metric == METRIC_HAMMING) e = exact_launch_any_t<hamming_b1_t<2>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_TANIMOTO || ix.metric == METRIC_JACCARD) e = exact_launch_any_t<tanimoto_b1_t<2>>(tiled, ix, a, swap, grid, smem, stream);
-        else if (ix.metric == METRIC_SORENSEN) e = exact_launch_any_t<sorensen_b1_t<2>>(tiled, ix, a, swap, grid, smem, stream);
+        if (ix.metric == METRIC_HAMMING) e = exact_launch_any_t<hamming_b1_t<2>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_TANIMOTO || ix.metric == METRIC_JACCARD) e = exact_launch_any_t<tanimoto_b1_t<2>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
+        else if (ix.metric == METRIC_SORENSEN) e = exact_launch_any_t<sorensen_b1_t<2>>(tiled, ix, a, swap, is_listed, grid, smem, stream);
         break;
     default: break;
     }
@@ -575,6 +622,27 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
         exact_merge_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, stream>>>(ix, a);
     if (cudaGetLastError() != cudaSuccess) return "CUDA failure: exact merge launch";
     return nullptr;
+}
+
+char const* exact_search_device(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t query_stride, size_t k,
+                                bool swap, bool slots_as_keys, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                                device_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
+    return exact_run(ix, sm_count, d_queries, nq, query_stride, k, swap, slots_as_keys, nullptr, d_keys, d_dists, d_counts, scratch, stream);
+}
+
+char const* exact_listed_queries_per_item(device_index_t const& ix, size_t k, uint32_t* qpc) {
+    device_buffer_t<uint8_t> unused;
+    exact_listed_t plan_only;
+    if (char const* e = exact_run(ix, 0, nullptr, 1, 0, k, false, false, &plan_only, nullptr, nullptr, nullptr, unused, nullptr)) return e;
+    *qpc = plan_only.qpc;
+    return nullptr;
+}
+
+char const* exact_listed_search_device(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t k,
+                                       exact_listed_t const& listed, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                                       device_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
+    exact_listed_t l = listed;
+    return exact_run(ix, sm_count, d_queries, nq, ix.vec_stride, k, false, false, &l, d_keys, d_dists, d_counts, scratch, stream);
 }
 
 } // namespace usearch_b200

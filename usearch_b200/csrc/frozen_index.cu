@@ -67,6 +67,7 @@ void frozen_index_t::release_device() {
     key_map.clear();
     key_table = key_table_t{};
     group_bits = device_buffer_t<uint32_t>{};
+    exact_filter = exact_filter_scratch_t{};
     keys_generation += 1;
 }
 

@@ -22,6 +22,8 @@
 
 namespace usearch_b200 {
 
+struct exact_item_t; /* exact_args.h: one CTA row of a listed exact scan */
+
 /* kernel entry points (search_kernel.cu) */
 cudaError_t search_launch(device_index_t const& ix, search_args_t const& a, int blocks, size_t smem, cudaStream_t stream);
 cudaError_t search_occupancy(device_index_t const& ix, int* blocks_per_sm, size_t smem, bool grouped = false);
@@ -242,6 +244,23 @@ struct frozen_index_t {
                                              uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
                                              uint64_t* keys, float* dists, size_t* counts, uint64_t* computed, uint64_t* visited);
 
+    /* grouped_filter.cu, exact form: search_exact_ over the live slots of each query's set (LISTED exact kernels). `groups`
+     * may be NULL when group_count == 1. The scratch is counted by memory_usage and freed by clear. */
+    struct exact_filter_scratch_t {
+        device_buffer_t<uint32_t> rows, list_at, query_at, per_set, item_at, order, sorted, ids, groups, scalars, counts;
+        device_buffer_t<uint64_t> entry_counts, entry_at, words, words_sorted, keys;
+        device_buffer_t<exact_item_t> items;
+        device_buffer_t<uint8_t> temp, queries, exact;
+        device_buffer_t<float> dists;
+        size_t bytes() const;
+    } exact_filter;
+    char const* grouped_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                            uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
+                                            float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited, cudaStream_t s);
+    char const* grouped_exact_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                          uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
+                                          uint64_t* keys, float* dists, size_t* counts, uint64_t* computed);
+
     /* searches */
     /* grouped: plan for the GROUPED kernel (its occupancy) */
     char const* plan(uint32_t k, uint32_t visited_cap_override, launch_plan_t& plan, uint32_t ef_override = 0,
@@ -281,6 +300,19 @@ struct frozen_index_t {
 char const* exact_search_device(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t query_stride, size_t k,
                                 bool swap, bool slots_as_keys, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
                                 device_buffer_t<uint8_t>& scratch, cudaStream_t stream);
+/* exact filtered search (grouped_filter.cu): `n_items` CTA rows of queries sorted by set, each against its set's slot list
+ * (exact_item_t, exact_args.h), over `total_rows` listed slots; the queries are gathered into rows of vec_stride bytes */
+struct exact_listed_t {
+    exact_item_t const* items = nullptr;
+    uint32_t n_items = 0;
+    uint32_t const* rows = nullptr;
+    uint32_t total_rows = 0;
+    uint32_t qpc = 0; /* queries per item of the kernel chosen for (ix, k) */
+};
+char const* exact_listed_queries_per_item(device_index_t const& ix, size_t k, uint32_t* qpc);
+char const* exact_listed_search_device(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t k,
+                                       exact_listed_t const& listed, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                                       device_buffer_t<uint8_t>& scratch, cudaStream_t stream);
 char const* exact_search_free(void const* dataset, size_t dataset_count, size_t dataset_stride, void const* queries,
                               size_t queries_count, size_t queries_stride, uint32_t scalar, size_t dimensions, uint32_t metric,
                               size_t count, uint64_t* keys, size_t keys_stride, float* distances, size_t distances_stride);

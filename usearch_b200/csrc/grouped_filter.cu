@@ -7,13 +7,21 @@
  *  cost is O(total keys), never O(slots x sets). The GROUPED search kernels test row groups[qi] where the single-set
  *  kernels test their one bitmap. When the rows of all sets do not fit the `group_bitmap_mb` budget, the sets are served
  *  in rounds of consecutive set ids, each round's queries a contiguous slice of the query ids sorted by set.
+ *
+ *  The exact form (search_exact_ over only the allowed slots) turns every set into an ascending, duplicate-free list of
+ *  its live slots: one thread per entry counts the key's cells in the table, a scan places them, a second pass writes one
+ *  (set << 32 | slot) word per cell, and a radix sort plus a unique leave the lists back to back. The queries, sorted by
+ *  set and gathered, then run through the LISTED exact kernels, whose CTAs never mix sets (exact_kernel.cu).
  */
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <algorithm>
 
 #include "cuda_check.h"
 #include "device_keys.h"
+#include "exact_args.h"
 #include "frozen_index.h"
 
 namespace usearch_b200 {
@@ -24,6 +32,7 @@ char const* const ERR_SHARDED = "Grouped filtered search does not serve a sharde
 char const* const ERR_NO_SETS = "A batch of queries needs at least one key set";
 char const* const ERR_GROUP = "A query's key set index is out of range";
 char const* const ERR_OFFSETS = "Key set offsets must start at 0 and never decrease";
+char const* const ERR_NO_GROUPS = "Without a set index per query, there must be exactly one key set";
 
 enum : uint32_t { BAD_GROUP = 1, BAD_OFFSETS = 2 };
 
@@ -82,6 +91,112 @@ __global__ void round_bounds_kernel(uint32_t const* sorted, uint32_t nq, uint32_
         else hi = mid;
     }
     bounds[r] = lo;
+}
+
+/* ---- exact filtered search ---- */
+
+/* the first g of [lo, hi) with offsets[g + 1] > e: the set holding CSR entry e */
+__device__ __forceinline__ uint32_t set_of_entry(uint64_t const* offsets, uint32_t sets, uint64_t e) {
+    uint32_t lo = 1, hi = sets;
+    while (lo < hi) {
+        uint32_t const mid = (lo + hi) >> 1;
+        if (offsets[mid] > e) hi = mid;
+        else lo = mid + 1;
+    }
+    return lo - 1;
+}
+
+/* counts[e] = the live slots under set_keys[e]; the table holds no slot of the free key, so removed slots never count. The
+ * counts are 64-bit so that their scan sums in 64 bits (cub takes the sum's type from its input). */
+__global__ void listed_count_kernel(key_cell_t const* cells, uint64_t mask, uint64_t const* set_keys, size_t entries, uint64_t* counts) {
+    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < entries; e += (size_t)gridDim.x * blockDim.x) {
+        uint64_t c = 0;
+        key_table_for_each(cells, mask, set_keys[e], [&](uint32_t) { ++c; });
+        counts[e] = c;
+    }
+}
+
+/* words[at[e] ..] = (set << 32) | slot for every slot under set_keys[e] */
+__global__ void listed_write_kernel(key_cell_t const* cells, uint64_t mask, uint64_t const* offsets, uint32_t sets, uint64_t const* set_keys,
+                                    size_t entries, uint64_t const* at, uint64_t* words) {
+    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < entries; e += (size_t)gridDim.x * blockDim.x) {
+        uint64_t const set = set_of_entry(offsets, sets + 1, e);
+        uint64_t p = at[e];
+        key_table_for_each(cells, mask, set_keys[e], [&](uint32_t s) { words[p++] = set << 32 | s; });
+    }
+}
+
+/* rows[i] = the slot of unique word i, and slot 0 past the last one up to `bound` (every row a listed scan may size its
+ * self-dots by is a real slot); list_at[g] = the first word of set g or later, for g <= sets */
+__global__ void listed_rows_kernel(uint64_t const* words, uint32_t const* unique_count, uint32_t bound, uint32_t sets, uint32_t* rows,
+                                   uint32_t* list_at) {
+    uint32_t const n = *unique_count;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < bound; i += gridDim.x * blockDim.x) rows[i] = i < n ? (uint32_t)words[i] : 0u;
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g <= sets; g += gridDim.x * blockDim.x) {
+        uint32_t lo = 0, hi = n;
+        while (lo < hi) {
+            uint32_t const mid = (lo + hi) >> 1;
+            if ((words[mid] >> 32) < g) lo = mid + 1;
+            else hi = mid;
+        }
+        list_at[g] = lo;
+    }
+}
+
+/* query_at[g] = the first position of `sorted` (set ids of the queries, ascending) holding g or more; per_set[g] = the
+ * work items set g needs at `qpc` queries per item (per_set[sets] = 0, so an exclusive scan ends at the item count) */
+__global__ void listed_item_counts_kernel(uint32_t const* sorted, uint32_t nq, uint32_t sets, uint32_t qpc, uint32_t* query_at, uint32_t* per_set) {
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g <= sets; g += gridDim.x * blockDim.x) {
+        auto first = [&](uint32_t v) {
+            uint32_t lo = 0, hi = nq;
+            while (lo < hi) {
+                uint32_t const mid = (lo + hi) >> 1;
+                if (sorted[mid] < v) lo = mid + 1;
+                else hi = mid;
+            }
+            return lo;
+        };
+        uint32_t const a = first(g);
+        query_at[g] = a;
+        per_set[g] = g < sets ? (first(g + 1) - a + qpc - 1) / qpc : 0u;
+    }
+}
+
+__global__ void listed_items_kernel(uint32_t const* query_at, uint32_t const* item_at, uint32_t const* list_at, uint32_t sets, uint32_t qpc,
+                                    exact_item_t* items) {
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < sets; g += gridDim.x * blockDim.x) {
+        uint32_t const q0 = query_at[g], q1 = query_at[g + 1];
+        uint32_t at = item_at[g];
+        for (uint32_t q = q0; q < q1; q += qpc) items[at++] = exact_item_t{q, min(qpc, q1 - q), list_at[g], list_at[g + 1] - list_at[g]};
+    }
+}
+
+/* row p of `out` (vec_stride bytes, zero padded) = the first `bytes` of caller row order[p] */
+__global__ void listed_gather_queries_kernel(uint8_t const* queries, size_t stride, uint32_t const* order, uint32_t nq, uint32_t bytes,
+                                             uint32_t vec_stride, uint8_t* out) {
+    for (uint32_t p = blockIdx.x; p < nq; p += gridDim.x) {
+        uint8_t const* src = queries + (size_t)order[p] * stride;
+        uint8_t* dst = out + (size_t)p * vec_stride;
+        for (uint32_t b = threadIdx.x; b < vec_stride; b += blockDim.x) dst[b] = b < bytes ? src[b] : (uint8_t)0;
+    }
+}
+
+/* the merged rows, in set order, back to the caller's order; computed_distances = the length of the query's list */
+__global__ void listed_scatter_kernel(uint32_t const* order, uint32_t const* sorted, uint32_t const* list_at, uint32_t nq, uint32_t k,
+                                      uint64_t const* keys, float const* dists, uint32_t const* counts, uint64_t* out_keys, float* out_dists,
+                                      uint32_t* out_counts, uint32_t* out_computed, uint32_t* out_visited) {
+    for (uint32_t p = blockIdx.x; p < nq; p += gridDim.x) {
+        uint32_t const i = order[p];
+        for (uint32_t j = threadIdx.x; j < k; j += blockDim.x) {
+            out_keys[(size_t)i * k + j] = keys[(size_t)p * k + j];
+            out_dists[(size_t)i * k + j] = dists[(size_t)p * k + j];
+        }
+        if (threadIdx.x == 0) {
+            out_counts[i] = counts[p];
+            if (out_computed) out_computed[i] = list_at[sorted[p] + 1] - list_at[sorted[p]];
+            if (out_visited) out_visited[i] = 0;
+        }
+    }
 }
 
 } // namespace
@@ -253,6 +368,221 @@ char const* frozen_index_t::grouped_filtered_search_host(void const* q, size_t n
         if (counts_out) counts_out[i] = h_counts.ptr[i];
         if (computed_out) computed_out[i] = h_computed.ptr[i];
         if (visited_out) visited_out[i] = h_cycles.ptr[i];
+    }
+    return nullptr;
+}
+
+/* ---------------------------------------------------------------------------------------------- */
+/*  exact filtered search: search_exact_ over the live slots of each query's key set              */
+/* ---------------------------------------------------------------------------------------------- */
+
+size_t frozen_index_t::exact_filter_scratch_t::bytes() const {
+    return entry_counts.capacity * 8 + entry_at.capacity * 8 + words.capacity * 8 + words_sorted.capacity * 8 + rows.capacity * 4 +
+           list_at.capacity * 4 + query_at.capacity * 4 + per_set.capacity * 4 + item_at.capacity * 4 + items.capacity * sizeof(exact_item_t) +
+           order.capacity * 4 + sorted.capacity * 4 + ids.capacity * 4 + groups.capacity * 4 + scalars.capacity * 4 + temp.capacity +
+           queries.capacity + keys.capacity * 8 + dists.capacity * 4 + counts.capacity * 4 + exact.capacity;
+}
+
+char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                                        uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
+                                                        float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                                        cudaStream_t s) {
+    if (shards) return ERR_SHARDED;
+    if (char const* e = ensure_context()) return e;
+    if (nq == 0 || k == 0) return nullptr;
+    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
+    if (group_count == 0) return ERR_NO_SETS;
+    if (group_count >= 0x7FFFFFFFull) return "Too many key sets in one call";
+    if (!groups && group_count != 1) return ERR_NO_GROUPS;
+    exact_filter_scratch_t& x = exact_filter;
+
+    /* every refusal comes before the first write to an output: the flag and the entry count in one read-back */
+    if (char const* e = group_flag.reserve(1)) return e;
+    CU(cudaMemsetAsync(group_flag.ptr, 0, 4, s));
+    grouped_validate_kernel<<<grid_for(std::max(nq, group_count), stream.sm_count), 256, 0, s>>>(groups, groups ? nq : 0, offsets, group_count,
+                                                                                                 group_flag.ptr);
+    CU(cudaGetLastError());
+    kernel_launches += 1;
+    uint32_t flag = 0;
+    uint64_t entries = 0;
+    CU(cudaMemcpyAsync(&flag, group_flag.ptr, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&entries, offsets + group_count, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (flag & BAD_GROUP) return ERR_GROUP;
+    if (flag & BAD_OFFSETS) return ERR_OFFSETS;
+    if (entries > 0x7FFFFFFFull) return "Too many keys in one call's sets";
+
+    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
+        CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
+        CU(cudaStreamSynchronize(s));
+        return nullptr;
+    }
+    uint32_t qpc = 0;
+    if (char const* e = exact_listed_queries_per_item(d, k, &qpc)) return e;
+    if (char const* e = ensure_key_table(s)) return e;
+    uint32_t const sets = (uint32_t)group_count;
+    size_t const n_entries = (size_t)entries;
+    auto temp_for = [&](size_t bytes) { return x.temp.reserve(std::max<size_t>(bytes, 1)); };
+    size_t temp_bytes = 0;
+
+    /* 1. the live slots of every entry, placed by an exclusive scan (one extra zero count: its place is the total) */
+    if (char const* e = x.entry_counts.reserve(n_entries + 1)) return e;
+    if (char const* e = x.entry_at.reserve(n_entries + 1)) return e;
+    if (char const* e = x.scalars.reserve(4)) return e;
+    CU(cudaMemsetAsync(x.entry_counts.ptr + n_entries, 0, 8, s));
+    if (n_entries)
+        listed_count_kernel<<<grid_for(n_entries, stream.sm_count), 256, 0, s>>>(key_table.cells.ptr, key_table.mask, set_keys, n_entries,
+                                                                                 x.entry_counts.ptr);
+    CU(cudaGetLastError());
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp_bytes, x.entry_counts.ptr, x.entry_at.ptr, (int)(n_entries + 1), s));
+    if (char const* e = temp_for(temp_bytes)) return e;
+    CU(cub::DeviceScan::ExclusiveSum(x.temp.ptr, temp_bytes, x.entry_counts.ptr, x.entry_at.ptr, (int)(n_entries + 1), s));
+    /* 2. the queries sorted by set, cut into work items of at most qpc queries that never mix sets (counted here, written
+     * once the lists are placed) */
+    if (char const* e = x.groups.reserve(nq)) return e;
+    if (char const* e = x.ids.reserve(nq)) return e;
+    if (char const* e = x.order.reserve(nq)) return e;
+    if (char const* e = x.sorted.reserve(nq)) return e;
+    if (char const* e = x.query_at.reserve(group_count + 1)) return e;
+    if (char const* e = x.per_set.reserve(group_count + 1)) return e;
+    if (char const* e = x.item_at.reserve(group_count + 1)) return e;
+    if (char const* e = x.items.reserve(nq)) return e;
+    if (!groups) { /* one set: every query uses set 0 */
+        CU(cudaMemsetAsync(x.groups.ptr, 0, nq * 4, s));
+        groups = x.groups.ptr;
+    }
+    iota_u32_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(x.ids.ptr, nq);
+    CU(cudaGetLastError());
+    int group_bits = 1;
+    while (group_bits < 32 && (group_count - 1) >> group_bits) ++group_bits;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, groups, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, group_bits, s));
+    if (char const* e = temp_for(temp_bytes)) return e;
+    CU(cub::DeviceRadixSort::SortPairs(x.temp.ptr, temp_bytes, groups, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, group_bits, s));
+    listed_item_counts_kernel<<<grid_for(group_count + 1, stream.sm_count), 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, sets, qpc, x.query_at.ptr,
+                                                                                         x.per_set.ptr);
+    CU(cudaGetLastError());
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp_bytes, x.per_set.ptr, x.item_at.ptr, (int)(group_count + 1), s));
+    if (char const* e = temp_for(temp_bytes)) return e;
+    CU(cub::DeviceScan::ExclusiveSum(x.temp.ptr, temp_bytes, x.per_set.ptr, x.item_at.ptr, (int)(group_count + 1), s));
+    /* one read-back: the cell total sizes the lists and the item count the grid. The total is an exact 64-bit sum (the
+     * counts are 64-bit), so a multi index whose sets name more than INT_MAX cells is refused here, before the sort (whose
+     * item count is an int) or any write to the lists. */
+    uint64_t cells = 0;
+    uint32_t n_items = 0;
+    CU(cudaMemcpyAsync(&cells, x.entry_at.ptr + n_entries, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&n_items, x.item_at.ptr + group_count, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (cells > 0x7FFFFFFFull) return "Too many listed rows in one call";
+
+    /* 3. (set << 32 | slot) words, sorted over the bits in use and deduplicated: per-set ascending slot lists */
+    int const n_cells = (int)cells;
+    int end_bit = 32;
+    while (end_bit < 64 && ((uint64_t)(sets - 1) >> (end_bit - 32))) ++end_bit;
+    if (char const* e = x.words.reserve(std::max<size_t>(cells, 1))) return e;
+    if (char const* e = x.words_sorted.reserve(std::max<size_t>(cells, 1))) return e;
+    if (char const* e = x.rows.reserve(std::max<size_t>(cells, 1))) return e;
+    if (char const* e = x.list_at.reserve(group_count + 1)) return e;
+    CU(cudaMemsetAsync(x.scalars.ptr, 0, 16, s));
+    if (n_cells) {
+        listed_write_kernel<<<grid_for(n_entries, stream.sm_count), 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, sets, set_keys,
+                                                                                 n_entries, x.entry_at.ptr, x.words.ptr);
+        CU(cudaGetLastError());
+        CU(cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, x.words.ptr, x.words_sorted.ptr, n_cells, 0, end_bit, s));
+        if (char const* e = temp_for(temp_bytes)) return e;
+        CU(cub::DeviceRadixSort::SortKeys(x.temp.ptr, temp_bytes, x.words.ptr, x.words_sorted.ptr, n_cells, 0, end_bit, s));
+        CU(cub::DeviceSelect::Unique(nullptr, temp_bytes, x.words_sorted.ptr, x.words.ptr, x.scalars.ptr, n_cells, s));
+        if (char const* e = temp_for(temp_bytes)) return e;
+        CU(cub::DeviceSelect::Unique(x.temp.ptr, temp_bytes, x.words_sorted.ptr, x.words.ptr, x.scalars.ptr, n_cells, s));
+        kernel_launches += 3;
+    }
+    listed_rows_kernel<<<grid_for(std::max<size_t>(cells, group_count + 1), stream.sm_count), 256, 0, s>>>(
+        x.words.ptr, x.scalars.ptr, (uint32_t)cells, sets, x.rows.ptr, x.list_at.ptr);
+    CU(cudaGetLastError());
+
+    listed_items_kernel<<<grid_for(group_count, stream.sm_count), 256, 0, s>>>(x.query_at.ptr, x.item_at.ptr, x.list_at.ptr, sets, qpc,
+                                                                               x.items.ptr);
+    CU(cudaGetLastError());
+    kernel_launches += 8;
+
+    /* 4. the gathered batch through the listed scans and the unchanged merge, then back to the caller's order */
+    size_t const vs = d.vec_stride;
+    if (char const* e = x.queries.reserve(nq * vs)) return e;
+    if (char const* e = x.keys.reserve(nq * k)) return e;
+    if (char const* e = x.dists.reserve(nq * k)) return e;
+    if (char const* e = x.counts.reserve(nq)) return e;
+    listed_gather_queries_kernel<<<(unsigned)std::min<size_t>(nq, 65535), 128, 0, s>>>(static_cast<uint8_t const*>(d_queries), stride,
+                                                                                       x.order.ptr, (uint32_t)nq, (uint32_t)d.bytes_per_vector,
+                                                                                       (uint32_t)vs, x.queries.ptr);
+    CU(cudaGetLastError());
+    exact_listed_t listed;
+    listed.items = x.items.ptr;
+    listed.n_items = n_items;
+    listed.rows = x.rows.ptr;
+    listed.total_rows = (uint32_t)cells; /* the lists' rows, duplicates still counted: the planner's bound */
+    CU(cudaEventRecord(ev_begin, s));
+    if (char const* e = exact_listed_search_device(d, stream.sm_count, x.queries.ptr, nq, k, listed, x.keys.ptr, x.dists.ptr, x.counts.ptr,
+                                                   x.exact, s))
+        return e;
+    CU(cudaEventRecord(ev_end, s));
+    listed_scatter_kernel<<<(unsigned)std::min<size_t>(nq, 65535), 128, 0, s>>>(x.order.ptr, x.sorted.ptr, x.list_at.ptr, (uint32_t)nq,
+                                                                                (uint32_t)k, x.keys.ptr, x.dists.ptr, x.counts.ptr, d_keys,
+                                                                                d_dists, d_counts, d_computed, d_visited);
+    CU(cudaGetLastError());
+    kernel_launches += 4;
+    CU(cudaStreamSynchronize(s));
+    CU(cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end));
+    return nullptr;
+}
+
+/* host queries of any kind, host sets and host outputs: checked here (the offsets size the upload), uploaded, and run through
+ * the device path, as grouped_filtered_search_host does */
+char const* frozen_index_t::grouped_exact_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                      uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
+                                                      uint64_t* keys, float* dists, size_t* counts_out, uint64_t* computed_out) {
+    std::lock_guard<std::mutex> lock(mutex);
+    if (shards) return ERR_SHARDED;
+    if (nq == 0 || k == 0) return nullptr;
+    if (group_count == 0) return ERR_NO_SETS;
+    if (!groups && group_count != 1) return ERR_NO_GROUPS;
+    if (offsets[0] != 0) return ERR_OFFSETS;
+    for (size_t g = 0; g < group_count; ++g)
+        if (offsets[g + 1] < offsets[g]) return ERR_OFFSETS;
+    if (groups)
+        for (size_t i = 0; i < nq; ++i)
+            if (groups[i] >= group_count) return ERR_GROUP;
+    if (!loaded || d.n == 0) { /* as exact_host answers on an empty index */
+        for (size_t i = 0; i < nq; ++i) {
+            for (size_t j = 0; j < k; ++j) { keys[i * k + j] = 0; reinterpret_cast<uint32_t*>(dists)[i * k + j] = SNAN_BITS; }
+            if (counts_out) counts_out[i] = 0;
+            if (computed_out) computed_out[i] = 0;
+        }
+        return nullptr;
+    }
+    if (char const* e = ensure_context()) return e;
+    size_t const vs = d.vec_stride ? d.vec_stride : 16, total = offsets[group_count];
+    if (char const* e = queries.reserve(nq * vs)) return e;
+    if (char const* e = out_keys.reserve(nq * k)) return e;
+    if (char const* e = out_dists.reserve(nq * k)) return e;
+    if (char const* e = counts_reserve_all(nq)) return e;
+    if (char const* e = group_upload.reserve(nq)) return e;
+    if (char const* e = group_offsets.reserve(group_count + 1)) return e;
+    if (char const* e = allowed_keys.reserve(std::max<size_t>(total, 1))) return e;
+    if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
+    if (groups) CU(cudaMemcpyAsync(group_upload.ptr, groups, nq * 4, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(group_offsets.ptr, offsets, (group_count + 1) * 8, cudaMemcpyHostToDevice, stream));
+    if (total) CU(cudaMemcpyAsync(allowed_keys.ptr, set_keys, total * 8, cudaMemcpyHostToDevice, stream));
+    if (char const* e = grouped_exact_search_device(queries.ptr, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count,
+                                                    allowed_keys.ptr, out_keys.ptr, out_dists.ptr, this->counts.ptr, computed.ptr, nullptr,
+                                                    stream))
+        return e;
+    CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_counts.ptr, this->counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_computed.ptr, computed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    for (size_t i = 0; i < nq; ++i) {
+        if (counts_out) counts_out[i] = h_counts.ptr[i];
+        if (computed_out) computed_out[i] = h_computed.ptr[i];
     }
     return nullptr;
 }

@@ -61,7 +61,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_get_many", "usearch_b200_export_keys", "usearch_b200_export_keys_at", "usearch_b200_copy",
     "usearch_b200_levels_stats", "usearch_b200_multi", "usearch_b200_count_many_device", "usearch_b200_get_many_device",
     "usearch_b200_filtered_search_many_device", "usearch_b200_grouped_filtered_search_many",
-    "usearch_b200_grouped_filtered_search_many_device",
+    "usearch_b200_grouped_filtered_search_many_device", "usearch_b200_grouped_filtered_exact_search_many",
+    "usearch_b200_grouped_filtered_exact_search_many_device",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -128,6 +129,14 @@ def load_library() -> C.CDLL:
                                                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                                      err]
+    lib.usearch_b200_grouped_filtered_exact_search_many.restype = C.c_size_t
+    lib.usearch_b200_grouped_filtered_exact_search_many.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int,
+                                                                    C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, err]
+    lib.usearch_b200_grouped_filtered_exact_search_many_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t,
+                                                                           C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                           C.c_void_p, C.c_void_p, err]
     lib.usearch_b200_tune.restype = C.c_int
     lib.usearch_b200_tune.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
     lib.usearch_b200_launch_plan.restype = C.c_int
@@ -742,14 +751,24 @@ class Index:
             return "i8"
         return kind
 
-    def filtered_search(self, vectors: np.ndarray, count: int, allowed_keys) -> Union[Matches, BatchMatches]:
-        """`filtered_search` (index_dense.hpp:774-779) for the predicate "key in allowed_keys"."""
-        return self.search(vectors, count, stats=True, _allowed=np.ascontiguousarray(allowed_keys, dtype=np.uint64))
+    def filtered_search(self, vectors: np.ndarray, count: int, allowed_keys, *, exact: bool = False) -> Union[Matches, BatchMatches]:
+        """`filtered_search` (index_dense.hpp:774-779) for the predicate "key in allowed_keys". `exact=True` scans exactly
+        the live entries whose key is allowed (search_exact_ with the predicate), on the GPU."""
+        if exact and np.ndim(allowed_keys) != 1:  # a scalar is a key, not a set; a nested list is several sets
+            raise ValueError("allowed_keys must be a flat sequence of keys")
+        allowed = np.ascontiguousarray(allowed_keys, dtype=np.uint64)
+        if not exact:
+            return self.search(vectors, count, stats=True, _allowed=allowed)
+        vectors = np.asarray(vectors)
+        nq = vectors.shape[0] if vectors.ndim == 2 else 1
+        return self._exact_sets(vectors, count, np.array([0, allowed.size], dtype=np.uint64), allowed, None, nq)
 
-    def grouped_filtered_search(self, vectors: np.ndarray, count: int, key_sets, groups=None) -> Union[Matches, BatchMatches]:
+    def grouped_filtered_search(self, vectors: np.ndarray, count: int, key_sets, groups=None, *,
+                                exact: bool = False) -> Union[Matches, BatchMatches]:
         """`filtered_search` with a key set per query, as one launch: row i equals
-        ``filtered_search(vectors[i], count, key_sets[groups[i]])``, counters included (`last_computed` / `last_visited`).
-        `key_sets` is a sequence of key iterables or arrays; ``groups=None`` gives query i the set i."""
+        ``filtered_search(vectors[i], count, key_sets[groups[i]], exact=exact)``, counters included (`last_computed` /
+        `last_visited`). `key_sets` is a sequence of key iterables or arrays; ``groups=None`` gives query i the set i.
+        `exact=True` scans exactly the live entries of each query's set."""
         vectors = np.asarray(vectors)
         single = vectors.ndim == 1
         if single:
@@ -777,6 +796,8 @@ class Index:
         offsets = np.zeros(len(sets) + 1, dtype=np.uint64)
         offsets[1:] = np.cumsum([len(keys) for keys in sets]) if sets else []
         flat = np.concatenate(sets) if sets else np.zeros(0, dtype=np.uint64)
+        if exact:
+            return self._exact_sets(vectors[0] if single else vectors, count, offsets, flat, groups, nq)
         if not vectors.flags.c_contiguous and vectors.strides[1] != vectors.itemsize:
             vectors = np.ascontiguousarray(vectors)
         kind = self._kind_of(vectors)
@@ -798,6 +819,34 @@ class Index:
             n = int(counts[0])
             return Matches(keys[0, :n], distances[0, :n], vm, cd)
         return BatchMatches(keys, distances, counts, vm, cd)
+
+    def _exact_sets(self, vectors: np.ndarray, count: int, offsets: np.ndarray, flat: np.ndarray, groups, nq: int):
+        """usearch_b200_grouped_filtered_exact_search_many over CSR sets; ``groups=None`` with one set means set 0 for all."""
+        single = vectors.ndim == 1
+        if single:
+            vectors = vectors[None, :]
+        if vectors.ndim != 2:
+            raise ValueError("Expects a matrix or a vector")
+        if not vectors.flags.c_contiguous and vectors.strides[1] != vectors.itemsize:
+            vectors = np.ascontiguousarray(vectors)
+        kind = self._kind_of(vectors)
+        keys = np.zeros((nq, count), dtype=np.uint64)
+        distances = np.zeros((nq, count), dtype=np.float32)
+        counts = np.zeros(nq, dtype=np.uint64)
+        computed = np.zeros(nq, dtype=np.uint64)
+        err = C.c_char_p()
+        self._lib.usearch_b200_grouped_filtered_exact_search_many(
+            self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count,
+            None if groups is None else groups.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), offsets.size - 1,
+            flat.ctypes.data_as(C.c_void_p), keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p),
+            counts.ctypes.data_as(C.c_void_p), computed.ctypes.data_as(C.c_void_p), C.byref(err))
+        _raise(err)
+        self.last_computed, self.last_visited = computed, np.zeros(nq, dtype=np.uint64)
+        cd = int(computed.sum())
+        if single:
+            n = int(counts[0])
+            return Matches(keys[0, :n], distances[0, :n], 0, cd)
+        return BatchMatches(keys, distances, counts, 0, cd)
 
     def cluster(self, vectors: np.ndarray, level: int = 1, *, stats: bool = False):
         """`index_dense_gt::cluster(vector, level)` (index_dense.hpp:788-793; index.hpp:3092-3125) for every row: the
@@ -1008,10 +1057,21 @@ class Index:
 
     def filtered_search_device(self, queries_ptr: int, nq: int, stride: int, count: int, allowed_ptr: int, allowed_count: int,
                                keys_ptr: int, distances_ptr: int, counts_ptr: int, computed_ptr: int = 0, visited_ptr: int = 0,
-                               stream: int = 0) -> None:
+                               stream: int = 0, *, exact: bool = False) -> None:
         """`search_device` restricted to `allowed_count` keys held in DEVICE memory (uint64): the result of
-        `filtered_search` with the same keys."""
+        `filtered_search` with the same keys (and the same `exact`). An exact search visits no graph members: it takes no
+        `visited_ptr`."""
         err = C.c_char_p()
+        if exact:
+            if visited_ptr:
+                raise ValueError("exact search has no visited_members counter")
+            import torch  # the one-set CSR offsets {0, allowed_count} live in device memory as well
+            offsets = torch.tensor([0, allowed_count], dtype=torch.int64, device=torch.device("cuda", self._lib.usearch_b200_device(self._h)))
+            self._lib.usearch_b200_grouped_filtered_exact_search_many_device(
+                self._h, queries_ptr, nq, stride, count, None, offsets.data_ptr(), 1, allowed_ptr or None, keys_ptr, distances_ptr,
+                counts_ptr, computed_ptr or None, stream or None, C.byref(err))
+            _raise(err)
+            return
         self._lib.usearch_b200_filtered_search_many_device(self._h, queries_ptr, nq, stride, count, allowed_ptr or None,
                                                            allowed_count, keys_ptr, distances_ptr, counts_ptr,
                                                            computed_ptr or None, visited_ptr or None, stream or None,
@@ -1020,10 +1080,19 @@ class Index:
 
     def grouped_filtered_search_device(self, queries_ptr: int, nq: int, stride: int, count: int, groups_ptr: int, offsets_ptr: int,
                                        sets_count: int, set_keys_ptr: int, keys_ptr: int, distances_ptr: int, counts_ptr: int,
-                                       computed_ptr: int = 0, visited_ptr: int = 0, stream: int = 0) -> None:
+                                       computed_ptr: int = 0, visited_ptr: int = 0, stream: int = 0, *, exact: bool = False) -> None:
         """`grouped_filtered_search` on DEVICE memory: queries in the index's kind, `groups` (uint32 [nq]), `offsets`
-        (uint64 [sets_count + 1]) and `set_keys` (uint64), outputs laid out as in `search_device`."""
+        (uint64 [sets_count + 1]) and `set_keys` (uint64), outputs laid out as in `search_device`. With `exact=True`,
+        `groups_ptr` may be 0 when `sets_count` is 1, and there is no `visited_ptr`."""
         err = C.c_char_p()
+        if exact:
+            if visited_ptr:
+                raise ValueError("exact search has no visited_members counter")
+            self._lib.usearch_b200_grouped_filtered_exact_search_many_device(
+                self._h, queries_ptr, nq, stride, count, groups_ptr or None, offsets_ptr or None, sets_count, set_keys_ptr or None,
+                keys_ptr, distances_ptr, counts_ptr, computed_ptr or None, stream or None, C.byref(err))
+            _raise(err)
+            return
         self._lib.usearch_b200_grouped_filtered_search_many_device(self._h, queries_ptr, nq, stride, count, groups_ptr or None,
                                                                    offsets_ptr or None, sets_count, set_keys_ptr or None, keys_ptr,
                                                                    distances_ptr, counts_ptr, computed_ptr or None,
