@@ -290,10 +290,12 @@ static int bm_pair_order(void const* x, void const* y) {
     return a->index < b->index ? -1 : a->index > b->index;
 }
 
-static int bm_candidate_order(void const* x, void const* y) { /* ascending distance, ties by slot */
+static int bm_candidate_order(void const* x, void const* y) { /* ascending distance, NaN after every number, ties by slot */
     candidate_t const* a = (candidate_t const*)x;
     candidate_t const* b = (candidate_t const*)y;
-    if (a->distance != b->distance) return a->distance < b->distance ? -1 : 1;
+    int const na = a->distance != a->distance, nb = b->distance != b->distance;
+    if (na != nb) return na ? 1 : -1;
+    if (!na && a->distance != b->distance) return a->distance < b->distance ? -1 : 1;
     return a->slot < b->slot ? -1 : a->slot > b->slot;
 }
 

@@ -301,7 +301,7 @@ __global__ void __launch_bounds__(LINK_THREADS, 3) link_reverse_kernel(__grid_co
         /* refine_ over the list plus the arrivals (index.hpp:3876-3890) */
         for (uint32_t i = threadIdx.x; i < LINK_CAND_MAX; i += blockDim.x) {
             uint32_t s = EMPTY_SLOT;
-            float d = __int_as_float(0x7f800000);
+            float d = __int_as_float(0x7fffffff); /* padding: a NaN with the largest slot sorts after everything */
             if (i < listed) s = row[i];
             else if (i < listed + arrivals) {
                 uint32_t const idx = a.sorted_idx[arrival[i - listed]];
@@ -321,8 +321,14 @@ __global__ void __launch_bounds__(LINK_THREADS, 3) link_reverse_kernel(__grid_co
             block_distances<M>(ix, q4, qc, cs, listed, cd, 0.f);
         }
         __syncthreads();
-        /* ascending by distance: bitonic sort of the LINK_CAND_MAX padded entries, one per thread */
+        /* ascending by distance, ties by slot, NaN after every number (DESIGN.md 3.5): bitonic sort of the LINK_CAND_MAX
+         * padded entries, one per thread */
         static_assert(LINK_CAND_MAX == LINK_THREADS, "one candidate per thread in the sort");
+        auto after = [](float da, uint32_t sa, float db, uint32_t sb) { /* (da, sa) sorts after (db, sb) */
+            bool const na = da != da, nb = db != db;
+            if (na != nb) return na;
+            return (!na && da > db) || ((na || da == db) && sa > sb);
+        };
         for (uint32_t size = 2; size <= LINK_CAND_MAX; size <<= 1) {
             for (uint32_t step = size >> 1; step > 0; step >>= 1) {
                 uint32_t const i = threadIdx.x, j = i ^ step;
@@ -330,7 +336,7 @@ __global__ void __launch_bounds__(LINK_THREADS, 3) link_reverse_kernel(__grid_co
                     bool const up = (i & size) == 0;
                     float const di = cd[i], dj = cd[j];
                     uint32_t const si = cs[i], sj = cs[j];
-                    bool const swap = up ? (di > dj || (di == dj && si > sj)) : (di < dj || (di == dj && si < sj));
+                    bool const swap = up ? after(di, si, dj, sj) : after(dj, sj, di, si);
                     if (swap) { cd[i] = dj; cd[j] = di; cs[i] = sj; cs[j] = si; }
                 }
                 __syncthreads();

@@ -127,11 +127,13 @@ struct heap_t {
 
     /*
      *  The same pop by the whole warp, for heaps whose internal nodes all sit in shared memory
-     *  (size <= 2*32*WORDS and size < smem_cap). shift_down follows, from the root, the child chosen by
-     *  `less`: right iff (right exists && right.d < left.d), else left — a choice that does not depend on
-     *  the element being sifted — and stops at the first level where the sifted element is not worse
-     *  (last.d > child.d fails); see index.hpp:819-834: `best` starts as last.d, moves to le.d if
-     *  last.d > le.d, then to re.d if best > re.d, which is exactly "last.d > min-child.d, ties to the left".
+     *  (size <= 2*32*WORDS and size < smem_cap). shift_down (index.hpp:819-834) keeps `best` = last.d, moves
+     *  it to le.d if last.d > le.d, then to re.d if best > re.d. With le.d a number that sends the element
+     *  right iff re.d < min(last.d, le.d), i.e. iff re.d < le.d and last.d > re.d; with le.d NaN the first
+     *  test fails, best stays last.d, and it goes right iff last.d > re.d. So the child it can take is fixed
+     *  by the two children alone: right iff (right exists && (re.d < le.d || le.d is NaN)), else left
+     *  (heap_goes_right, search_order.h), and the element moves there iff last.d > child.d. The walk follows
+     *  those choices from the root and stops at the first level where last.d > child.d fails:
      *    1. every lane evaluates the choice bit of up to WORDS internal nodes, one per 32-node word the heap reaches:
      *       one 16-byte load and one ballot each;
      *    2. all lanes walk the <= 9 levels on those bits in registers (no memory on the critical path);
@@ -160,7 +162,7 @@ struct heap_t {
                     asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
                                  : "=f"(le.d), "=r"(le.s), "=f"(re.d), "=r"(re.s)
                                  : "r"(smem_addr + 16u * p));
-                    right = re.d < le.d;
+                    right = heap_goes_right(le.d, re.d);
                 }
                 w[r] = __ballot_sync(0xffffffffu, right);
             }
@@ -204,16 +206,22 @@ struct heap_t {
 /* sorted_buffer_gt::insert(element, limit) (index.hpp:928-939). Uniform across the warp.
  * Lane l owns elements l, l+32, ...: every element is loaded once (the same loads feed the
  * lower_bound ballots), one barrier, then every element at or after the insertion point is
- * stored one place to the right. */
+ * stored one place to the right. `has_nan` (uniform) says `top` may hold a NaN: the count of
+ * smaller elements is lower_bound only while it does not, so then the position is probed as
+ * libstdc++ probes it (search_order.h). */
 __device__ __forceinline__ void top_insert(float* td, uint32_t* ts, uint32_t& size, uint32_t limit, float d, uint32_t s,
-                                           int lane) {
+                                           bool& has_nan, int lane) {
     uint32_t pos = 0;
-    for (uint32_t b = 0; b < size; b += 32) {
-        uint32_t i = b + lane;
-        bool lt = i < size && td[i] < d;
-        pos += __popc(__ballot_sync(0xffffffffu, lt));
-    }
+    if (!has_nan) {
+        for (uint32_t b = 0; b < size; b += 32) {
+            uint32_t i = b + lane;
+            bool lt = i < size && td[i] < d;
+            pos += __popc(__ballot_sync(0xffffffffu, lt));
+        }
+    } else
+        pos = probe_lower_bound([td](uint32_t i) { return td[i]; }, size, d);
     if (pos == limit) return;
+    has_nan = top_may_hold_nan(has_nan, d);
     bool full = size == limit;
     uint32_t hi = size - (full ? 1u : 0u);
     if (hi > pos) {
@@ -712,6 +720,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
         return ix.upper + ((size_t)ub + (uint32_t)(bl - 1)) * ix.m_stride;
     };
     uint32_t top_size = 0, heap_size = 0, computed = 0, cycles = 0, status = STATUS_OK;
+    bool top_nan = false; /* `top` may hold a NaN: its inserts probe as lower_bound does */
     uint32_t visited_total = 0;
     bool log_overflow_out = false;
     bool const prof = a.phase_cycles != nullptr;
@@ -871,6 +880,7 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
                     if (lane == 0) { rtd[0] = radius; rts[0] = closest; }
                 } else if (lane == 0) { top_d[0] = radius; top_s[0] = closest; }
                 top_size = 1;
+                top_nan = top_may_hold_nan(false, radius);
             }
         }
         __syncwarp();
@@ -1031,10 +1041,10 @@ __device__ __forceinline__ void search_one(device_index_t const& ix, search_args
                         bool allowed = insert ? s != qi : GROUPED ? slot_allowed_row(ix, group_row, s) : slot_allowed(ix, a, s);
                         if (allowed) {
                             if (topreg) {
-                                top_insert_reg(rtd, rts, top_size, ef, d, s, lane);
+                                top_insert_reg(rtd, rts, top_size, ef, d, s, top_nan, lane);
                                 radius = top_back_reg(rtd, top_size);
                             } else {
-                                top_insert(top_d, top_s, top_size, ef, d, s, lane);
+                                top_insert(top_d, top_s, top_size, ef, d, s, top_nan, lane);
                                 radius = top_d[top_size - 1];
                             }
                         }

@@ -7,6 +7,8 @@
 
 #include <cstdint>
 
+#include "search_order.h"
+
 namespace usearch_b200 {
 
 /* ---- TMA bulk copy + mbarrier (PTX ISA: cp.async.bulk, mbarrier.*) ---------------------------- */
@@ -46,14 +48,31 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, void const* src, uin
  */
 constexpr int TOP_E = 8;
 
-__device__ __forceinline__ void top_insert_reg(float (&td)[TOP_E], uint32_t (&ts)[TOP_E], uint32_t& size, uint32_t limit,
-                                               float d, uint32_t s, int lane) {
-    uint32_t const g0 = (uint32_t)lane * TOP_E;
-    uint32_t mine = 0; /* lower_bound: number of stored distances strictly below d */
+/* element g of a register `top`: register g % TOP_E of lane g / TOP_E; every lane calls it with the same g */
+__device__ __forceinline__ float top_at_reg(float const (&td)[TOP_E], uint32_t g) {
+    uint32_t const r = g & (TOP_E - 1);
+    float sel = td[0];
 #pragma unroll
-    for (int j = 0; j < TOP_E; ++j) mine += (g0 + j < size && td[j] < d) ? 1u : 0u;
-    uint32_t const pos = __reduce_add_sync(0xffffffffu, mine);
+    for (int j = 1; j < TOP_E; ++j)
+        if ((uint32_t)j == r) sel = td[j];
+    return __shfl_sync(0xffffffffu, sel, (int)(g / TOP_E));
+}
+
+/* `has_nan` (uniform): `top` may hold a NaN, and only the probe of libstdc++'s lower_bound places d as the
+ * reference does (search_order.h); without one, the count of smaller elements is that position */
+__device__ __forceinline__ void top_insert_reg(float (&td)[TOP_E], uint32_t (&ts)[TOP_E], uint32_t& size, uint32_t limit,
+                                               float d, uint32_t s, bool& has_nan, int lane) {
+    uint32_t const g0 = (uint32_t)lane * TOP_E;
+    uint32_t pos;
+    if (!has_nan) {
+        uint32_t mine = 0; /* lower_bound: number of stored distances strictly below d */
+#pragma unroll
+        for (int j = 0; j < TOP_E; ++j) mine += (g0 + j < size && td[j] < d) ? 1u : 0u;
+        pos = __reduce_add_sync(0xffffffffu, mine);
+    } else
+        pos = probe_lower_bound([&td](uint32_t g) { return top_at_reg(td, g); }, size, d);
     if (pos == limit) return;
+    has_nan = top_may_hold_nan(has_nan, d);
     bool const full = size == limit;
     uint32_t const hi = size - (full ? 1u : 0u); /* old [pos, hi) becomes new (pos, hi] */
     float const up_d = __shfl_up_sync(0xffffffffu, td[TOP_E - 1], 1);
@@ -73,14 +92,7 @@ __device__ __forceinline__ void top_insert_reg(float (&td)[TOP_E], uint32_t (&ts
 }
 
 /* distance of the last (worst) element: sorted_buffer_gt::top() (index.hpp:891) */
-__device__ __forceinline__ float top_back_reg(float const (&td)[TOP_E], uint32_t size) {
-    uint32_t const i = size - 1, r = i & (TOP_E - 1);
-    float sel = td[0];
-#pragma unroll
-    for (int j = 1; j < TOP_E; ++j)
-        if ((uint32_t)j == r) sel = td[j];
-    return __shfl_sync(0xffffffffu, sel, (int)(i / TOP_E));
-}
+__device__ __forceinline__ float top_back_reg(float const (&td)[TOP_E], uint32_t size) { return top_at_reg(td, size - 1); }
 
 /* The same insert under the TOTAL order (distance ascending, slot descending): what a sequence of
  * sorted_buffer_gt::insert calls in ascending slot order converges to (each equal distance is placed BEFORE
