@@ -539,6 +539,31 @@ inline index_dense_t::state_result_t index_dense_t::copy() const {
     return state;
 }
 
+/* usearch_exact_search: brute force over a raw host matrix, keys are dataset row numbers (exact_search_t,
+ * index_plugins.hpp:2071-2164). Strides in bytes; the dataset may exceed GPU memory. `threads` host threads stage it. */
+template <typename scalar_at>
+inline error_t exact_search(scalar_at const* dataset, std::size_t dataset_size, std::size_t dataset_stride, scalar_at const* queries,
+                            std::size_t queries_size, std::size_t queries_stride, std::size_t dimensions, usearch_metric_kind_t metric,
+                            std::size_t wanted, vector_key_t* keys, std::size_t keys_stride, distance_t* distances,
+                            std::size_t distances_stride, std::size_t threads = 0) {
+    usearch_error_t e = nullptr;
+    usearch_exact_search(dataset, dataset_size, dataset_stride, queries, queries_size, queries_stride, scalar_kind<scalar_at>(), dimensions,
+                         metric, wanted, threads, keys, keys_stride, distances, distances_stride, &e);
+    return e;
+}
+
+/* the same over DEVICE arrays, enqueued on `cuda_stream` (a cudaStream_t; nullptr = the default stream) without waiting */
+inline error_t exact_search_device(void const* dataset, std::size_t dataset_size, std::size_t dataset_stride, void const* queries,
+                                   std::size_t queries_size, std::size_t queries_stride, usearch_scalar_kind_t scalar,
+                                   std::size_t dimensions, usearch_metric_kind_t metric, std::size_t wanted, vector_key_t* keys,
+                                   std::size_t keys_stride, distance_t* distances, std::size_t distances_stride,
+                                   void* cuda_stream = nullptr) {
+    usearch_error_t e = nullptr;
+    usearch_b200_exact_search_device(dataset, dataset_size, dataset_stride, queries, queries_size, queries_stride, scalar, dimensions,
+                                     metric, wanted, keys, keys_stride, distances, distances_stride, cuda_stream, &e);
+    return e;
+}
+
 /* metadata is taken from the file */
 inline index_dense_t::state_result_t index_dense_t::make(char const* path, bool view) {
     state_result_t state;

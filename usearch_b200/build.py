@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libusearch_b200.so")
-SOURCES = ["c_abi.cu", "frozen_index.cu", "search_kernel.cu", "exact_kernel.cu", "exact_imma.cu", "exact_wgmma.cu", "builder.cu", "shards.cu", "join.cu", "indexes.cu", "surface.cu", "device_keys.cu", "grouped_filter.cu"]
+SOURCES = ["c_abi.cu", "frozen_index.cu", "search_kernel.cu", "exact_kernel.cu", "exact_imma.cu", "exact_wgmma.cu", "builder.cu", "shards.cu", "join.cu", "indexes.cu", "surface.cu", "device_keys.cu", "grouped_filter.cu", "exact_free.cu"]
 HEADERS = ["device_index.h", "frozen_index.h", "metrics.cuh", "warp_primitives.cuh", "exact_args.h", "exact_i8.h", "key_map.h", "device_keys.h", "prefilter_bound.h", "search_order.h",
            "join_resolve.h", "cuda_check.h", "cuda_buffers.h", "f64_casts.h", "scalar_casts.h", os.path.join("..", "..", "include", "usearch_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -717,12 +717,27 @@ usearch_distance_t usearch_distance(void const* a, void const* b, usearch_scalar
 
 void usearch_exact_search(void const* dataset, size_t dataset_size, size_t dataset_stride, void const* queries, size_t queries_size,
                           size_t queries_stride, usearch_scalar_kind_t scalar_kind, size_t dimensions, usearch_metric_kind_t metric_kind,
-                          size_t count, size_t /*threads*/, usearch_key_t* keys, size_t keys_stride, usearch_distance_t* distances,
+                          size_t count, size_t threads, usearch_key_t* keys, size_t keys_stride, usearch_distance_t* distances,
                           size_t distances_stride, usearch_error_t* error) {
     uint32_t const m = metric_to_char(metric_kind), s = scalar_to_char(scalar_kind);
     if (!m || !s) return set_error(error, "Unknown metric kind!");
-    set_error(error, exact_search_free(dataset, dataset_size, dataset_stride, queries, queries_size, queries_stride, s, dimensions, m, count,
-                                       keys, keys_stride, distances, distances_stride));
+    set_error(error, guarded([&] {
+        return exact_search_free(dataset, dataset_size, dataset_stride, queries, queries_size, queries_stride, s, dimensions, m, count, threads,
+                                 keys, keys_stride, distances, distances_stride);
+    }));
+}
+
+/* usearch_exact_search over device matrices, in the caller's stream (exact_free.cu) */
+void usearch_b200_exact_search_device(void const* dataset, size_t dataset_size, size_t dataset_stride, void const* queries,
+                                      size_t queries_size, size_t queries_stride, usearch_scalar_kind_t scalar_kind, size_t dimensions,
+                                      usearch_metric_kind_t metric_kind, size_t count, usearch_key_t* keys, size_t keys_stride,
+                                      usearch_distance_t* distances, size_t distances_stride, void* cuda_stream, usearch_error_t* error) {
+    uint32_t const m = metric_to_char(metric_kind), s = scalar_to_char(scalar_kind);
+    if (!m || !s) return set_error(error, "Unknown metric kind!");
+    set_error(error, guarded([&] {
+        return exact_search_free_device(dataset, dataset_size, dataset_stride, queries, queries_size, queries_stride, s, dimensions, m, count,
+                                        keys, keys_stride, distances, distances_stride, static_cast<cudaStream_t>(cuda_stream));
+    }));
 }
 
 /* index_dense_gt::cluster(vector, level) (index_dense.hpp:788-793 -> cluster_ :2088-2109 -> index.hpp:3092-3125) for a

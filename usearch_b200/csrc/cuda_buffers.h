@@ -1,6 +1,6 @@
 /*
- *  cuda_buffers.h — owners of the CUDA resources the host side holds: device and pinned host buffers, a stream with its
- *  device, and events. Each frees what it holds when it is destroyed or assigned over, and can be moved but not
+ *  cuda_buffers.h — owners of the CUDA resources the host side holds: device and pinned host buffers, device buffers
+ *  taken and given back in stream order, a stream with its device, and events. Each frees what it holds when it is destroyed or assigned over, and can be moved but not
  *  copied, so no code keeps a list of what to free. Plain C++ against the runtime API: tests/native/test_cuda_buffers.cpp
  *  compiles it with g++ and a counting stand-in for the runtime.
  */
@@ -60,6 +60,39 @@ template <typename T, bool Pinned> struct cuda_buffer_t {
 template <typename T> using device_buffer_t = cuda_buffer_t<T, false>;
 template <typename T> using pinned_buffer_t = cuda_buffer_t<T, true>;
 
+/* `capacity` elements of T in device memory taken and given back in the order of `stream` (cudaMallocAsync /
+ * cudaFreeAsync), for a call that owns scratch but must not wait for its stream: the memory returns to the pool only
+ * after the work enqueued on `stream` before the release. */
+template <typename T> struct stream_buffer_t {
+    T* ptr = nullptr;
+    size_t capacity = 0; /* elements */
+    cudaStream_t stream = nullptr;
+
+    explicit stream_buffer_t(cudaStream_t s) : stream(s) {}
+    stream_buffer_t(stream_buffer_t const&) = delete;
+    stream_buffer_t& operator=(stream_buffer_t const&) = delete;
+    ~stream_buffer_t() { release(); }
+
+    /* room for at least `n` elements; growing does not keep the contents. On failure the buffer is empty. */
+    char const* reserve(size_t n) {
+        if (n <= capacity) return nullptr;
+        release();
+        void* p = nullptr;
+        if (cudaMallocAsync(&p, n * sizeof(T), stream) != cudaSuccess) {
+            cudaGetLastError();
+            return "Out of GPU memory!";
+        }
+        ptr = static_cast<T*>(p);
+        capacity = n;
+        return nullptr;
+    }
+    void release() {
+        if (ptr) cudaFreeAsync(ptr, stream);
+        ptr = nullptr;
+        capacity = 0;
+    }
+};
+
 /* one runtime handle, destroyed with `destroy` */
 template <typename H, cudaError_t (*destroy)(H)> struct cuda_handle_t {
     H handle = nullptr;
@@ -89,6 +122,11 @@ struct cuda_event_t : cuda_handle_t<cudaEvent_t, cudaEventDestroy> {
     cudaError_t create() {
         release();
         return cudaEventCreate(&handle);
+    }
+    /* the same with cudaEventCreateWithFlags (cudaEventDisableTiming for events that only order streams) */
+    cudaError_t create(unsigned int flags) {
+        release();
+        return cudaEventCreateWithFlags(&handle, flags);
     }
 };
 

@@ -341,8 +341,11 @@ __global__ void __launch_bounds__(TILED_WARPS * 32, 1) exact_tiled_kernel(__grid
     }
 }
 
-/* one warp per query: merge the per-segment lists under (distance asc, slot desc), map slots to keys, pad */
-__global__ void exact_merge_kernel(device_index_t ix, exact_args_t a) {
+/* one warp per query: merge the per-segment lists under (distance asc, slot desc), map slots to keys, pad.
+ * A free search over a dataset in chunks (exact_free.cu) scans one chunk per launch: `row_offset` turns the chunk's rows
+ * into dataset rows, and with `carry` the output row already holds the merged list of the chunks before (slots as keys),
+ * which is merged as one more segment. The order is total, so any cut of the dataset gives the same list. */
+__global__ void exact_merge_kernel(device_index_t ix, exact_args_t a, uint32_t row_offset, bool carry) {
     uint32_t const qi = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int const lane = threadIdx.x & 31;
     if (qi >= a.nq) return;
@@ -351,11 +354,19 @@ __global__ void exact_merge_kernel(device_index_t ix, exact_args_t a) {
 #pragma unroll
     for (int j = 0; j < TOP_E; ++j) { td[j] = 0.f; ts[j] = 0u; }
     uint32_t top_size = 0;
+    if (carry) {
+        uint32_t const n = a.out_counts[qi];
+        size_t const row = (size_t)qi * a.k;
+        for (uint32_t i = 0; i < n; ++i)
+            top_insert_reg_keyed(td, ts, top_size, a.k, a.out_dists[row + i], (uint32_t)a.out_keys[row + i], lane);
+    }
     for (uint32_t seg = 0; seg < a.segments; ++seg) {
         uint32_t const n = a.part_n[(size_t)qi * a.segments + seg];
         size_t const row = ((size_t)qi * a.segments + seg) * a.k;
-        for (uint32_t i = 0; i < n; ++i) top_insert_reg_keyed(td, ts, top_size, a.k, a.part_d[row + i], a.part_s[row + i], lane);
+        for (uint32_t i = 0; i < n; ++i)
+            top_insert_reg_keyed(td, ts, top_size, a.k, a.part_d[row + i], a.part_s[row + i] + row_offset, lane);
     }
+    __syncwarp(); /* every lane has read the carried row before any lane overwrites it */
 #pragma unroll
     for (int j = 0; j < TOP_E; ++j) {
         uint32_t const i = (uint32_t)lane * TOP_E + (uint32_t)j;
@@ -374,7 +385,8 @@ __global__ void exact_merge_kernel(device_index_t ix, exact_args_t a) {
 }
 
 /* the same merge for count > 256: the merged list lives in global memory (L2) instead of registers */
-__global__ void exact_merge_big_kernel(device_index_t ix, exact_args_t a, float* merged_d, uint32_t* merged_s) {
+__global__ void exact_merge_big_kernel(device_index_t ix, exact_args_t a, float* merged_d, uint32_t* merged_s, uint32_t row_offset,
+                                       bool carry) {
     uint32_t const qi = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int const lane = threadIdx.x & 31;
     if (qi >= a.nq) return;
@@ -382,13 +394,17 @@ __global__ void exact_merge_big_kernel(device_index_t ix, exact_args_t a, float*
     uint32_t* ms = merged_s + (size_t)qi * a.k;
     uint32_t top_size = 0;
     float worst = 0.f;
+    if (carry) /* the chunks before, ascending like a segment's list; it cannot overflow the empty list */
+        for (uint32_t i = 0, n = a.out_counts[qi]; i < n; ++i)
+            top_insert_global_keyed(md, ms, top_size, a.k, a.out_dists[(size_t)qi * a.k + i], (uint32_t)a.out_keys[(size_t)qi * a.k + i], lane);
+    if (top_size == a.k) worst = reinterpret_cast<float volatile*>(md)[a.k - 1];
     for (uint32_t seg = 0; seg < a.segments; ++seg) {
         uint32_t const n = a.part_n[(size_t)qi * a.segments + seg];
         size_t const row = ((size_t)qi * a.segments + seg) * a.k;
         for (uint32_t i = 0; i < n; ++i) {
             float const cd = a.part_d[row + i];
             if (top_size == a.k && cd > worst) break; /* the segment's list is ascending: nothing later can enter */
-            top_insert_global_keyed(md, ms, top_size, a.k, cd, a.part_s[row + i], lane);
+            top_insert_global_keyed(md, ms, top_size, a.k, cd, a.part_s[row + i] + row_offset, lane);
             if (top_size == a.k) worst = reinterpret_cast<float volatile*>(md)[a.k - 1];
         }
     }
@@ -467,10 +483,12 @@ static int exact_lpv(device_index_t const& ix) {
  *  Scratch for the per-segment partial lists is taken from `scratch` (grown on demand).
  *  `listed` (exact filtered search, swap = false): the CTAs serve its work items against their slot lists instead; with
  *  `listed->items == nullptr` nothing runs and `listed->qpc` receives the queries per item of the kernel that would.
+ *  `row_offset` and `carry`: one chunk of a free search (exact_merge_kernel).
  */
+template <class scratch_at>
 static char const* exact_run(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t query_stride, size_t k,
                              bool swap, bool slots_as_keys, exact_listed_t* listed, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
-                             device_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
+                             scratch_at& scratch, cudaStream_t stream, uint32_t row_offset = 0, bool carry = false) {
     if (!nq || !k) return nullptr;
     /* count <= 256: k-best lists in registers (scan, IMMA, merge); beyond that the tiled kernel's global-memory lists and
      * exact_merge_big_kernel carry any count (search_exact_ takes any `wanted`, index.hpp:4251-4268) */
@@ -616,10 +634,10 @@ static char const* exact_run(device_index_t const& ix, int sm_count, void const*
     if (e != cudaSuccess) return "CUDA failure: exact scan launch";
     if (big_k) {
         float* merged_d = reinterpret_cast<float*>(scratch.ptr + norms_at);
-        exact_merge_big_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, stream>>>(ix, a, merged_d,
-                                                                                      reinterpret_cast<uint32_t*>(merged_d + nq * k));
+        exact_merge_big_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, stream>>>(
+            ix, a, merged_d, reinterpret_cast<uint32_t*>(merged_d + nq * k), row_offset, carry);
     } else
-        exact_merge_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, stream>>>(ix, a);
+        exact_merge_kernel<<<(unsigned)((nq * 32 + 255) / 256), 256, 0, stream>>>(ix, a, row_offset, carry);
     if (cudaGetLastError() != cudaSuccess) return "CUDA failure: exact merge launch";
     return nullptr;
 }
@@ -628,6 +646,18 @@ char const* exact_search_device(device_index_t const& ix, int sm_count, void con
                                 bool swap, bool slots_as_keys, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
                                 device_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
     return exact_run(ix, sm_count, d_queries, nq, query_stride, k, swap, slots_as_keys, nullptr, d_keys, d_dists, d_counts, scratch, stream);
+}
+
+char const* exact_search_chunk_device(device_index_t const& chunk, int sm_count, void const* d_queries, size_t nq, size_t query_stride,
+                                      size_t k, uint32_t row_offset, bool carry, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                                      stream_buffer_t<uint8_t>& scratch, cudaStream_t stream) {
+    return exact_run(chunk, sm_count, d_queries, nq, query_stride, k, true, true, nullptr, d_keys, d_dists, d_counts, scratch, stream,
+                     row_offset, carry);
+}
+
+char const* exact_search_check(device_index_t const& shape, size_t k) {
+    uint32_t qpc = 0;
+    return exact_listed_queries_per_item(shape, k, &qpc);
 }
 
 char const* exact_listed_queries_per_item(device_index_t const& ix, size_t k, uint32_t* qpc) {

@@ -313,9 +313,22 @@ char const* exact_listed_queries_per_item(device_index_t const& ix, size_t k, ui
 char const* exact_listed_search_device(device_index_t const& ix, int sm_count, void const* d_queries, size_t nq, size_t k,
                                        exact_listed_t const& listed, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
                                        device_buffer_t<uint8_t>& scratch, cudaStream_t stream);
+/* one chunk of a free search (exact_free.cu): metric(row, query), keys are dataset rows `row_offset + chunk row`; with `carry`
+ * the outputs already hold the merged top-k of the chunks before and are merged with this one */
+char const* exact_search_chunk_device(device_index_t const& chunk, int sm_count, void const* d_queries, size_t nq, size_t query_stride,
+                                      size_t k, uint32_t row_offset, bool carry, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                                      stream_buffer_t<uint8_t>& scratch, cudaStream_t stream);
+/* the refusals exact_search_device would return for this shape (metric, scalar kind, row length) and count, nothing launched */
+char const* exact_search_check(device_index_t const& shape, size_t k);
+
+/* exact_free.cu: usearch_exact_search over host rows (any count of them), and its twin over device rows */
 char const* exact_search_free(void const* dataset, size_t dataset_count, size_t dataset_stride, void const* queries,
                               size_t queries_count, size_t queries_stride, uint32_t scalar, size_t dimensions, uint32_t metric,
-                              size_t count, uint64_t* keys, size_t keys_stride, float* distances, size_t distances_stride);
+                              size_t count, size_t threads, uint64_t* keys, size_t keys_stride, float* distances, size_t distances_stride);
+char const* exact_search_free_device(void const* dataset, size_t dataset_count, size_t dataset_stride, void const* queries,
+                                     size_t queries_count, size_t queries_stride, uint32_t scalar, size_t dimensions, uint32_t metric,
+                                     size_t count, uint64_t* keys, size_t keys_stride, float* distances, size_t distances_stride,
+                                     cudaStream_t stream);
 
 /* shards.cu */
 char const* shards_unique_id(void* out128);
