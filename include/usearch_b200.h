@@ -258,6 +258,7 @@ bool usearch_b200_multi(usearch_index_t index);
  * every rank receives the merged rows. Collective: all ranks must call with the same queries and count. */
 void usearch_b200_shards_unique_id(void* unique_id128, usearch_error_t* error);
 void usearch_b200_shards_join(usearch_index_t index, int rank, int world, void const* unique_id128, usearch_error_t* error);
+/* Host buffers. Returns the sum of counts over the merged rows, whether or not `counts` is NULL. */
 size_t usearch_b200_sharded_search_many(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                         usearch_scalar_kind_t query_kind, size_t count, usearch_key_t* keys,
                                         usearch_distance_t* distances, size_t* counts, usearch_error_t* error);
@@ -413,7 +414,9 @@ size_t usearch_b200_search_many_stats(usearch_index_t index, void const* queries
 /* Device-side counterpart of usearch_filtered_search (usearch.h:391-395) for the one predicate family that
  * can run on a GPU: "the key is in this set". `allowed_keys` (host memory, any order, may be empty) is turned
  * into a bitmap over slots; the predicate is applied where the reference applies its callback
- * (index_dense.hpp:2078-2083, index.hpp:4201/4236): rejected members are still traversed, never returned. */
+ * (index_dense.hpp:2078-2083, index.hpp:4201/4236): rejected members are still traversed, never returned. The keys are
+ * sorted on the device, as usearch_b200_filtered_search_many_device sorts them, so more than INT_MAX of them are refused
+ * with its error. Returns the sum of counts. */
 size_t usearch_b200_filtered_search_many(usearch_index_t index, void const* queries, size_t queries_count,
                                          size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
                                          usearch_key_t const* allowed_keys, size_t allowed_count, usearch_key_t* keys,
@@ -430,7 +433,8 @@ void usearch_b200_cluster_many(usearch_index_t index, void const* queries, size_
 
 /* `search(exact = true)` of the reference's C++ / Python surface (index.hpp:3047-3051, search_exact_ :4251-4268) for a
  * batch: brute force over every non-removed member of the frozen index, ties resolved exactly like the reference's
- * sequence of sorted inserts (equal distances: larger slot first). Any count; beyond 256 the lists live in L2 instead of registers. */
+ * sequence of sorted inserts (equal distances: larger slot first). Any count; beyond 256 the lists live in L2 instead of registers.
+ * Returns the sum of counts, whether or not `counts` is NULL. */
 size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries, size_t queries_count,
                                       size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
                                       usearch_key_t* keys, usearch_distance_t* distances, size_t* counts,

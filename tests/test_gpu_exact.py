@@ -122,6 +122,30 @@ def test_free_exact_search_rejects_more_neighbours_than_rows():
         exact_search(base, q, 6, metric="l2sq")
 
 
+def test_exact_and_sharded_host_entries_return_the_total_without_counts():
+    """usearch_b200_exact_search_many and usearch_b200_sharded_search_many (one shard) return the sum of counts, whether or
+    not the caller passes `counts`."""
+    import ctypes as C
+    import os
+    from usearch_b200.index import SCALAR_KIND, Index
+    index = Index.restore(np.load(os.path.join(common.GOLDEN, "cos_f32_n2000_d64.npz"))["blob"])
+    index.join_shards(0, 1, bytes(128))
+    q = np.random.default_rng(5).standard_normal((50, 64), dtype=np.float32)
+    k = 10
+    for entry in (index._lib.usearch_b200_exact_search_many, index._lib.usearch_b200_sharded_search_many):
+        totals = []
+        for counts in (np.zeros(len(q), np.uint64), None):
+            keys, dists = np.zeros((len(q), k), np.uint64), np.zeros((len(q), k), np.float32)
+            err = C.c_char_p()
+            totals.append(entry(index._h, q.ctypes.data_as(C.c_void_p), len(q), q.strides[0], SCALAR_KIND["f32"], k,
+                                keys.ctypes.data_as(C.c_void_p), dists.ctypes.data_as(C.c_void_p),
+                                None if counts is None else counts.ctypes.data_as(C.c_void_p), C.byref(err)))
+            assert err.value is None
+            if counts is not None:
+                assert totals[0] == int(counts.sum()) == len(q) * k
+        assert totals[1] == totals[0]
+
+
 @pytest.mark.parametrize("metric,scalar,n,d,m", [
     ("cos", "f32", 6000, 768, 4),      # STAGED kernel
     ("l2sq", "f32", 6000, 32, 4),      # DIRECT kernel

@@ -14,7 +14,6 @@
 #include <algorithm>
 #include <cstring>
 #include <new>
-#include <utility>
 #include <vector>
 
 #include "../../include/usearch_b200.h"
@@ -94,8 +93,27 @@ void set_error(usearch_error_t* error, char const* message) {
     if (error && message) *error = message;
 }
 
-template <class... A> char const* search_host_guarded(frozen_index_t* ix, A&&... args) {
-    return guarded([&] { return ix->search_host(std::forward<A>(args)...); });
+/* a search entry on host buffers: `run(query scalar, &total)` under `guarded`; returns the sum of counts, 0 on an error */
+template <class F> size_t host_search(usearch_scalar_kind_t query_kind, usearch_error_t* error, F&& run) {
+    uint32_t const qs = scalar_to_char(query_kind);
+    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
+    size_t total = 0;
+    if (char const* e = guarded([&] { return run(qs, &total); })) {
+        set_error(error, e);
+        return 0;
+    }
+    return total;
+}
+
+/* an entry on device buffers: `run(ix, stream)` under the handle's lock and `guarded`, with its context, on the caller's
+ * stream (NULL = the handle's own) */
+template <class F> void device_search(usearch_index_t index, void* cuda_stream, usearch_error_t* error, F&& run) {
+    frozen_index_t* ix = as_index(index);
+    std::lock_guard<std::mutex> lock(ix->mutex);
+    set_error(error, guarded([&]() -> char const* {
+        if (char const* e = ix->ensure_context()) return e;
+        return run(ix, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
+    }));
 }
 
 /* read-only mapping of a file, handed to load_blob */
@@ -272,16 +290,10 @@ void usearch_change_metric(usearch_index_t, usearch_metric_t, void*, usearch_met
 
 size_t usearch_search(usearch_index_t index, void const* query, usearch_scalar_kind_t query_kind, size_t count,
                       usearch_key_t* keys, usearch_distance_t* distances, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    size_t total = 0;
     /* concurrent single-query callers are coalesced into one launch (frozen_index_t::search_single) */
-    if (char const* e = guarded([&] { return ix->search_single(query, qs, count, keys, distances, &total); })) {
-        set_error(error, e);
-        return 0;
-    }
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->search_single(query, qs, count, keys, distances, total);
+    });
 }
 
 /* usearch.h:391-395, c/lib.cpp:413-429. A host callback cannot run inside the kernel; it is evaluated on the host once per
@@ -292,52 +304,36 @@ size_t usearch_filtered_search(usearch_index_t index, void const* query, usearch
                                usearch_distance_t* distances, usearch_error_t* error) {
     if (!filter) return usearch_search(index, query, query_kind, count, keys, distances, error);
     frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    std::vector<uint64_t> allowed;
-    {
-        std::lock_guard<std::mutex> lock(ix->mutex);
-        for (uint64_t key : ix->host_keys)
-            if (key != ix->free_key && filter(key, filter_state)) allowed.push_back(key);
-    }
-    size_t total = 0;
-    if (char const* e = search_host_guarded(ix, query, 1, 0, qs, count, keys, count * 8, distances, count * 4, nullptr, nullptr,
-                                        nullptr, &total, allowed.data(), allowed.size(), true)) {
-        set_error(error, e);
-        return 0;
-    }
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        std::vector<uint64_t> allowed;
+        {
+            std::lock_guard<std::mutex> lock(ix->mutex);
+            for (uint64_t key : ix->host_keys)
+                if (key != ix->free_key && filter(key, filter_state)) allowed.push_back(key);
+        }
+        return ix->filtered_search_host(query, 1, 0, qs, count, allowed.data(), allowed.size(), host_results_t{keys, count * 8, distances, count * 4},
+                                        total);
+    });
 }
 
 size_t usearch_search_many(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                            usearch_scalar_kind_t query_kind, size_t count, usearch_key_t* keys, size_t keys_stride,
                            usearch_distance_t* distances, size_t distances_stride, size_t* counts, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    size_t total = 0;
-    if (char const* e = search_host_guarded(ix, queries, queries_count, queries_stride, qs, count, keys, keys_stride, distances,
-                                        distances_stride, counts, nullptr, nullptr, &total)) {
-        set_error(error, e);
-        return 0;
-    }
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->search_host(queries, queries_count, queries_stride, qs, count,
+                                            host_results_t{keys, keys_stride, distances, distances_stride, counts}, total);
+    });
 }
 
 size_t usearch_b200_search_many_stats(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                       usearch_scalar_kind_t query_kind, size_t count, usearch_key_t* keys,
                                       usearch_distance_t* distances, size_t* counts, uint64_t* computed_distances,
                                       uint64_t* visited_members, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    size_t total = 0;
-    if (char const* e = search_host_guarded(ix, queries, queries_count, queries_stride, qs, count, keys, count * 8, distances,
-                                        count * 4, counts, computed_distances, visited_members, &total)) {
-        set_error(error, e);
-        return 0;
-    }
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->search_host(queries, queries_count, queries_stride, qs, count,
+                                            host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances, visited_members},
+                                            total);
+    });
 }
 
 size_t usearch_b200_filtered_search_many(usearch_index_t index, void const* queries, size_t queries_count,
@@ -345,54 +341,37 @@ size_t usearch_b200_filtered_search_many(usearch_index_t index, void const* quer
                                          usearch_key_t const* allowed_keys, size_t allowed_count, usearch_key_t* keys,
                                          usearch_distance_t* distances, size_t* counts, uint64_t* computed_distances,
                                          uint64_t* visited_members, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    size_t total = 0;
-    if (char const* e = search_host_guarded(ix, queries, queries_count, queries_stride, qs, count, keys, count * 8, distances,
-                                        count * 4, counts, computed_distances, visited_members, &total, allowed_keys,
-                                        allowed_count, true)) {
-        set_error(error, e);
-        return 0;
-    }
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->filtered_search_host(queries, queries_count, queries_stride, qs, count, allowed_keys, allowed_count,
+                                                     host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances,
+                                                                    visited_members},
+                                                     total);
+    });
 }
 
 void usearch_b200_search_many_device(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                      size_t count, usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                      uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                      usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    if (char const* e = ix->ensure_context()) return set_error(error, e);
-    cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream;
-    set_error(error, ix->search_device(queries, queries_count, queries_stride, count, keys, distances, counts,
-                                       computed_distances, visited_members, s));
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
+        return ix->search_device(queries, queries_count, queries_stride, count, keys, distances, counts, computed_distances, visited_members, s);
+    });
 }
 
 /* lookups by key from device memory (device_keys.cu), on the caller's stream like usearch_b200_search_many_device */
 void usearch_b200_count_many_device(usearch_index_t index, usearch_key_t const* keys, size_t count, uint32_t* counts,
                                     void* cuda_stream, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    set_error(error, guarded([&]() -> char const* {
-        if (char const* e = ix->ensure_context()) return e;
-        return ix->count_many_device(keys, count, counts, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
-    }));
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) { return ix->count_many_device(keys, count, counts, s); });
 }
 
 void usearch_b200_get_many_device(usearch_index_t index, usearch_key_t const* keys, size_t count, size_t max_per_key,
                                   void* vectors, size_t vectors_stride, usearch_scalar_kind_t kind, uint32_t* counts,
                                   void* cuda_stream, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    set_error(error, guarded([&]() -> char const* {
-        if (char const* e = ix->ensure_context()) return e;
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) -> char const* {
         uint32_t const vs = scalar_to_char(kind);
         if (!vs) return "Unknown scalar kind!";
-        return ix->get_many_device(keys, count, max_per_key, vectors, vectors_stride, vs, counts,
-                                   cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
-    }));
+        return ix->get_many_device(keys, count, max_per_key, vectors, vectors_stride, vs, counts, s);
+    });
 }
 
 void usearch_b200_filtered_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
@@ -400,14 +379,10 @@ void usearch_b200_filtered_search_many_device(usearch_index_t index, void const*
                                               size_t allowed_count, usearch_key_t* keys, usearch_distance_t* distances,
                                               uint32_t* counts, uint32_t* computed_distances, uint32_t* visited_members,
                                               void* cuda_stream, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    set_error(error, guarded([&]() -> char const* {
-        if (char const* e = ix->ensure_context()) return e;
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
         return ix->filtered_search_device(queries, queries_count, queries_stride, count, allowed_keys, allowed_count, keys, distances,
-                                          counts, computed_distances, visited_members,
-                                          cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
-    }));
+                                          counts, computed_distances, visited_members, s);
+    });
 }
 
 /* grouped filtered search (grouped_filter.cu): query i filtered by key set groups[i] of a CSR list of sets */
@@ -417,21 +392,13 @@ size_t usearch_b200_grouped_filtered_search_many(usearch_index_t index, void con
                                                  usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
                                                  size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
                                                  usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    std::vector<size_t> own(counts ? 0 : queries_count);
-    size_t* const found = counts ? counts : own.data();
-    if (char const* e = guarded([&] {
-            return ix->grouped_filtered_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count, set_keys,
-                                                    keys, distances, found, computed_distances, visited_members);
-        })) {
-        set_error(error, e);
-        return 0;
-    }
-    size_t total = 0;
-    for (size_t i = 0; i < queries_count && count; ++i) total += found[i];
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->grouped_filtered_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count,
+                                                             set_keys,
+                                                             host_results_t{keys, count * 8, distances, count * 4, counts,
+                                                                            computed_distances, visited_members},
+                                                             total);
+    });
 }
 
 void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
@@ -440,14 +407,10 @@ void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, voi
                                                       usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                                       uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                                       usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    set_error(error, guarded([&]() -> char const* {
-        if (char const* e = ix->ensure_context()) return e;
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
         return ix->grouped_filtered_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
-                                                  keys, distances, counts, computed_distances, visited_members,
-                                                  cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
-    }));
+                                                  keys, distances, counts, computed_distances, visited_members, s);
+    });
 }
 
 /* exact filtered search (grouped_filter.cu): search_exact_ over only the live slots of each query's key set */
@@ -456,21 +419,12 @@ size_t usearch_b200_grouped_filtered_exact_search_many(usearch_index_t index, vo
                                                        uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
                                                        usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
                                                        size_t* counts, uint64_t* computed_distances, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    std::vector<size_t> own(counts ? 0 : queries_count);
-    size_t* const found = counts ? counts : own.data();
-    if (char const* e = guarded([&] {
-            return ix->grouped_exact_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count, set_keys, keys,
-                                                 distances, found, computed_distances);
-        })) {
-        set_error(error, e);
-        return 0;
-    }
-    size_t total = 0;
-    for (size_t i = 0; i < queries_count && count; ++i) total += found[i];
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->grouped_exact_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count,
+                                                          set_keys,
+                                                          host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances},
+                                                          total);
+    });
 }
 
 void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
@@ -478,14 +432,10 @@ void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t inde
                                                             uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
                                                             usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                                             uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    set_error(error, guarded([&]() -> char const* {
-        if (char const* e = ix->ensure_context()) return e;
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
         return ix->grouped_exact_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys, keys,
-                                               distances, counts, computed_distances, nullptr,
-                                               cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream);
-    }));
+                                               distances, counts, computed_distances, nullptr, s);
+    });
 }
 
 /* the asynchronous pair: enqueue any number of batches (kernel launches only, nothing waits), then finish once */
@@ -493,12 +443,10 @@ void usearch_b200_search_many_enqueue(usearch_index_t index, void const* queries
                                       size_t count, usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                       uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                       usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    if (char const* e = ix->ensure_context()) return set_error(error, e);
-    cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream;
-    set_error(error, ix->search_device(queries, queries_count, queries_stride, count, keys, distances, counts, computed_distances,
-                                       visited_members, s, true));
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
+        return ix->search_device(queries, queries_count, queries_stride, count, keys, distances, counts, computed_distances, visited_members, s,
+                                 true);
+    });
 }
 
 void usearch_b200_search_many_finish(usearch_index_t index, usearch_error_t* error) {
@@ -745,27 +693,19 @@ void usearch_b200_exact_search_device(void const* dataset, size_t dataset_size, 
 void usearch_b200_cluster_many(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                usearch_scalar_kind_t query_kind, size_t level, usearch_key_t* keys, usearch_distance_t* distances,
                                uint64_t* computed_distances, uint64_t* visited_members, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) return set_error(error, "Unknown scalar kind!");
-    set_error(error, search_host_guarded(ix, queries, queries_count, queries_stride, qs, 1, keys, 8, distances, 4, nullptr, computed_distances,
-                                     visited_members, nullptr, nullptr, 0, false, (int)std::min<size_t>(level, 0x7FFF)));
+    host_search(query_kind, error, [&](uint32_t qs, size_t*) {
+        return as_index(index)->cluster_host(queries, queries_count, queries_stride, qs, level, keys, distances, computed_distances,
+                                             visited_members);
+    });
 }
 
 size_t usearch_b200_exact_search_many(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                       usearch_scalar_kind_t query_kind, size_t count, usearch_key_t* keys, usearch_distance_t* distances,
                                       size_t* counts, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    if (char const* e = ix->exact_host(queries, queries_count, queries_stride, qs, count, keys, distances, counts)) {
-        set_error(error, e);
-        return 0;
-    }
-    size_t total = 0;
-    if (counts)
-        for (size_t i = 0; i < queries_count; ++i) total += counts[i];
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->exact_host(queries, queries_count, queries_stride, qs, count,
+                                           host_results_t{keys, count * 8, distances, count * 4, counts}, total);
+    });
 }
 
 /* ---- sharded search: one process per GPU, one shard per process (python/lib.cpp:321-402 `Indexes`) ------------------ */
@@ -781,32 +721,23 @@ void usearch_b200_shards_join(usearch_index_t index, int rank, int world, void c
 size_t usearch_b200_sharded_search_many(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                         usearch_scalar_kind_t query_kind, size_t count, usearch_key_t* keys,
                                         usearch_distance_t* distances, size_t* counts, usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    uint32_t qs = scalar_to_char(query_kind);
-    if (!qs) { set_error(error, "Unknown scalar kind!"); return 0; }
-    if (char const* e = ix->sharded_search_host(queries, queries_count, queries_stride, qs, count, keys, distances, counts)) {
-        set_error(error, e);
-        return 0;
-    }
-    size_t total = 0;
-    if (counts)
-        for (size_t i = 0; i < queries_count; ++i) total += counts[i];
-    return total;
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->sharded_search_host(queries, queries_count, queries_stride, qs, count,
+                                                    host_results_t{keys, count * 8, distances, count * 4, counts}, total);
+    });
 }
 
 void usearch_b200_sharded_search_many_device(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                              size_t count, usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                              uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                              usearch_error_t* error) {
-    frozen_index_t* ix = as_index(index);
-    std::lock_guard<std::mutex> lock(ix->mutex);
-    if (char const* e = ix->ensure_context()) return set_error(error, e);
-    cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ix->stream;
-    char const* e = ix->sharded_search_device(queries, queries_count, queries_stride, count, keys, distances, counts,
-                                              computed_distances, visited_members, s);
-    /* on the handle's own stream the caller has nothing to order its next use of the outputs with: finish before returning */
-    if (!e && !cuda_stream && cudaStreamSynchronize(s) != cudaSuccess) e = "CUDA failure: synchronize";
-    set_error(error, e);
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
+        char const* e = ix->sharded_search_device(queries, queries_count, queries_stride, count, keys, distances, counts,
+                                                  computed_distances, visited_members, s);
+        /* on the handle's own stream the caller has nothing to order its next use of the outputs with: finish before returning */
+        if (!e && !cuda_stream && cudaStreamSynchronize(s) != cudaSuccess) e = "CUDA failure: synchronize";
+        return e;
+    });
 }
 
 size_t usearch_b200_shards_payload_bytes(size_t queries_count, size_t count) { return shards_payload_bytes(queries_count, count); }

@@ -2,7 +2,7 @@
  *  device_keys.cu — lookups by key for callers whose keys are already in HBM: count, get and filtered search. The first
  *  two probe the key -> slot table of device_keys.h, built from the device `keys` array on the first lookup after any
  *  change of the key -> slot relation (`keys_generation`); filtered search needs no table, it sorts the allowed keys on
- *  the device and builds the same slot bitmap as the host path.
+ *  the device and builds a bitmap over slots from them, for device keys and for host keys uploaded first.
  */
 #include <cub/device/device_radix_sort.cuh>
 
@@ -19,6 +19,8 @@ namespace {
 
 /* output bytes of one chunk of get_many_device when the chunk-row knob is 0, as in get_many */
 constexpr size_t GET_CHUNK_BYTES = 64ull << 20;
+
+char const* const ERR_TOO_MANY_ALLOWED = "Too many allowed keys in one call";
 
 struct claim_cas_t {
     __device__ bool operator()(uint32_t* word, uint32_t slot) const { return atomicCAS(word, EMPTY_SLOT, slot) == EMPTY_SLOT; }
@@ -202,17 +204,14 @@ char const* frozen_index_t::get_many_device(uint64_t const* keys, size_t n, size
 }
 
 /* usearch_b200_filtered_search_many with device queries, allowed keys and outputs: the allowed keys sorted on the device
- * into `allowed_keys`, the slot bitmap and the launch exactly as search_host builds and runs them */
+ * into `allowed_keys`, then the slot bitmap the search filters by */
 char const* frozen_index_t::filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t const* allowed,
                                                    size_t allowed_count, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
                                                    uint32_t* d_computed, uint32_t* d_visited, cudaStream_t s) {
     if (char const* e = ensure_context()) return e;
     if (nq == 0 || k == 0) return nullptr;
-    if (allowed_count > (size_t)INT_MAX) return "Too many allowed keys in one call";
-    struct reset_filter_t {
-        frozen_index_t* self;
-        ~reset_filter_t() { self->active_allow_bits = nullptr; }
-    } reset_filter{this};
+    if (allowed_count > (size_t)INT_MAX) return ERR_TOO_MANY_ALLOWED;
+    search_filter_t filter;
     if (loaded && size) {
         int const m = (int)allowed_count;
         if (char const* e = allowed_keys.reserve(std::max<size_t>(allowed_count, 1))) return e;
@@ -225,9 +224,24 @@ char const* frozen_index_t::filtered_search_device(void const* d_queries, size_t
             kernel_launches += 1;
         }
         CU(search_build_allow_bits(d, allowed_keys.ptr, (uint32_t)m, allow_bits.ptr, s));
-        active_allow_bits = allow_bits.ptr;
+        filter.allow_bits = allow_bits.ptr;
     }
-    return search_device(d_queries, nq, stride, k, d_keys, d_dists, d_counts, d_computed, d_visited, s);
+    return search_device(d_queries, nq, stride, k, d_keys, d_dists, d_counts, d_computed, d_visited, s, false, filter);
+}
+
+/* usearch_b200_filtered_search_many and usearch_filtered_search: the host keys staged on the device as given, then sorted
+ * and applied by filtered_search_device (cub's sort must not write over its input) */
+char const* frozen_index_t::filtered_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                 uint64_t const* allowed, size_t allowed_count, host_results_t const& out, size_t* total) {
+    if (nq == 0 || k == 0) return nullptr;
+    std::lock_guard<std::mutex> lock(mutex);
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    if (allowed_count > (size_t)INT_MAX) return ERR_TOO_MANY_ALLOWED; /* refused before 16 GiB of keys are uploaded */
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
+                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
+        if (char const* e = stage_keys(allowed, allowed_count)) return e;
+        return filtered_search_device(dq, nq, vs, k, key_stage.ptr, allowed_count, r.keys, r.dists, r.counts, r.computed, r.visited, stream);
+    });
 }
 
 } // namespace usearch_b200

@@ -563,7 +563,7 @@ char const* frozen_index_t::prepare_launch(launch_plan_t const& pl, size_t warps
 
 char const* frozen_index_t::search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t* d_keys,
                                           float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles,
-                                          cudaStream_t s, bool defer) {
+                                          cudaStream_t s, bool defer, search_filter_t const& filter) {
     if (nq == 0 || k == 0) return nullptr;
     if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
     if (char const* e = ensure_context()) return e;
@@ -602,8 +602,8 @@ char const* frozen_index_t::search_device(void const* d_queries, size_t nq, size
     a.out_computed = d_computed;
     a.out_visited = d_cycles;
     a.status = status_ptr;
-    a.allow_bits = active_allow_bits;
-    a.cluster_end_level = active_cluster_end_level;
+    a.allow_bits = filter.allow_bits;
+    a.cluster_end_level = filter.cluster_end_level;
 
     if (profile_phases) {
         if (char const* e = phase_cycles.reserve(PHASE_COUNTERS)) return e;
@@ -708,82 +708,82 @@ char const* frozen_index_t::upload_queries(void const* q, size_t nq, size_t stri
     return cast_rows_device(cast_stage.ptr, src_bytes, query_scalar, queries.ptr, vs, scalar, dimensions, nq, stream);
 }
 
-char const* frozen_index_t::search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                        uint64_t* keys, size_t keys_stride, float* dists, size_t dists_stride,
-                                        size_t* counts, uint64_t* computed_out, uint64_t* cycles_out, size_t* total,
-                                        uint64_t const* allowed, size_t allowed_count, bool filtered, int cluster_level) {
-    if (total) *total = 0;
-    if (nq == 0 || k == 0) return nullptr;
-    std::lock_guard<std::mutex> lock(mutex);
-    if (!loaded || d.n == 0) { /* index_gt::search on an empty index: no matches, no error (index.hpp:3036-3037) */
-        if (cluster_level >= 0) return "No clusters to identify";
-        for (size_t i = 0; i < nq; ++i) {
-            uint64_t* krow = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(keys) + i * keys_stride);
-            uint32_t* drow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(dists) + i * dists_stride);
-            for (size_t j = 0; j < k; ++j) { krow[j] = 0; drow[j] = SNAN_BITS; }
-            if (counts) counts[i] = 0;
-            if (computed_out) computed_out[i] = 0;
-            if (cycles_out) cycles_out[i] = 0;
-        }
-        return nullptr;
+char const* frozen_index_t::stage_keys(uint64_t const* keys, size_t n) {
+    if (char const* e = key_stage.reserve(std::max<size_t>(n, 1))) return e;
+    if (n) CU(cudaMemcpyAsync(key_stage.ptr, keys, n * 8, cudaMemcpyHostToDevice, stream));
+    return nullptr;
+}
+
+char const* answer_empty(size_t nq, size_t k, host_results_t const& out) {
+    for (size_t i = 0; i < nq; ++i) {
+        uint64_t* krow = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(out.keys) + i * out.keys_stride);
+        uint32_t* drow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(out.dists) + i * out.dists_stride);
+        for (size_t j = 0; j < k; ++j) { krow[j] = 0; drow[j] = SNAN_BITS; }
+        if (out.counts) out.counts[i] = 0;
+        if (out.computed) out.computed[i] = 0;
+        if (out.visited) out.visited[i] = 0;
     }
+    return nullptr;
+}
+
+char const* frozen_index_t::search_round_trip(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                              host_results_t const& out, size_t* total, device_search_t const& search) {
     if (char const* e = ensure_context()) return e;
     size_t const vs = d.vec_stride ? d.vec_stride : 16;
-
     if (char const* e = queries.reserve(nq * vs)) return e;
     if (char const* e = out_keys.reserve(nq * k)) return e;
     if (char const* e = out_dists.reserve(nq * k)) return e;
     if (char const* e = counts_reserve_all(nq)) return e;
     if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
-
-    /* filtered search: sort the allowed keys on the host, turn them into a bitmap over slots on the device */
-    struct reset_filter_t {
-        frozen_index_t* self;
-        ~reset_filter_t() { self->active_allow_bits = nullptr; self->active_cluster_end_level = -1; }
-    } reset_filter{this};
-    /* index_gt::cluster (index.hpp:3115-3116): levels max..`level`, with level 0 treated as level 1 */
-    if (cluster_level >= 0) active_cluster_end_level = cluster_level <= 0 ? 0 : cluster_level - 1;
-    if (filtered && size) {
-        std::vector<uint64_t> sorted(allowed, allowed + allowed_count);
-        std::sort(sorted.begin(), sorted.end());
-        if (char const* e = allowed_keys.reserve(std::max<size_t>(sorted.size(), 1))) return e;
-        if (char const* e = allow_bits.reserve((size + 31) / 32)) return e;
-        if (!sorted.empty())
-            CU(cudaMemcpyAsync(allowed_keys.ptr, sorted.data(), sorted.size() * 8, cudaMemcpyHostToDevice, stream));
-        CU(search_build_allow_bits(d, allowed_keys.ptr, (uint32_t)sorted.size(), allow_bits.ptr, stream));
-        CU(cudaStreamSynchronize(stream)); /* `sorted` is pageable host memory */
-        active_allow_bits = allow_bits.ptr;
-    }
-
-    bool const want_stats = computed_out || cycles_out;
-    if (char const* e = search_device(queries.ptr, nq, vs, k, out_keys.ptr, out_dists.ptr, this->counts.ptr,
-                                      want_stats ? computed.ptr : nullptr, want_stats ? cycles.ptr : nullptr, stream))
+    if (char const* e = search(queries.ptr, vs, device_results_t{out_keys.ptr, out_dists.ptr, counts.ptr, out.computed ? computed.ptr : nullptr,
+                                                                 out.visited ? cycles.ptr : nullptr}))
         return e;
 
-    /* results -> host */
-    bool const dense = keys_stride == k * 8 && dists_stride == k * 4;
-    if (dense) {
-        CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
+    if (out.keys_stride == k * 8 && out.dists_stride == k * 4) {
+        CU(cudaMemcpyAsync(out.keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
+        CU(cudaMemcpyAsync(out.dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
     } else {
-        CU(cudaMemcpy2DAsync(keys, keys_stride, out_keys.ptr, k * 8, k * 8, nq, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpy2DAsync(dists, dists_stride, out_dists.ptr, k * 4, k * 4, nq, cudaMemcpyDeviceToHost, stream));
+        CU(cudaMemcpy2DAsync(out.keys, out.keys_stride, out_keys.ptr, k * 8, k * 8, nq, cudaMemcpyDeviceToHost, stream));
+        CU(cudaMemcpy2DAsync(out.dists, out.dists_stride, out_dists.ptr, k * 4, k * 4, nq, cudaMemcpyDeviceToHost, stream));
     }
-    CU(cudaMemcpyAsync(h_counts.ptr, this->counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    if (want_stats) {
-        CU(cudaMemcpyAsync(h_computed.ptr, computed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(h_cycles.ptr, cycles.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    }
+    CU(cudaMemcpyAsync(h_counts.ptr, counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    if (out.computed) CU(cudaMemcpyAsync(h_computed.ptr, computed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+    if (out.visited) CU(cudaMemcpyAsync(h_cycles.ptr, cycles.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));
     size_t sum = 0;
     for (size_t i = 0; i < nq; ++i) {
         sum += h_counts.ptr[i];
-        if (counts) counts[i] = h_counts.ptr[i];
-        if (computed_out) computed_out[i] = h_computed.ptr[i];
-        if (cycles_out) cycles_out[i] = h_cycles.ptr[i];
+        if (out.counts) out.counts[i] = h_counts.ptr[i];
+        if (out.computed) out.computed[i] = h_computed.ptr[i];
+        if (out.visited) out.visited[i] = h_cycles.ptr[i];
     }
-    if (total) *total = sum;
+    *total = sum;
     return nullptr;
+}
+
+char const* frozen_index_t::search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                        host_results_t const& out, size_t* total) {
+    if (nq == 0 || k == 0) return nullptr;
+    std::lock_guard<std::mutex> lock(mutex);
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total, [&](void const* dq, size_t vs, device_results_t const& r) {
+        return search_device(dq, nq, vs, k, r.keys, r.dists, r.counts, r.computed, r.visited, stream);
+    });
+}
+
+/* index_gt::cluster (index.hpp:3115-3116): the greedy descent over levels max..`level`, with level 0 treated as level 1 */
+char const* frozen_index_t::cluster_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t level, uint64_t* keys,
+                                         float* dists, uint64_t* computed_out, uint64_t* visited_out) {
+    if (nq == 0) return nullptr;
+    std::lock_guard<std::mutex> lock(mutex);
+    if (!loaded || d.n == 0) return "No clusters to identify";
+    search_filter_t filter;
+    filter.cluster_end_level = level <= 1 ? 0 : (int)std::min<size_t>(level, 0x7FFF) - 1;
+    size_t total = 0;
+    host_results_t const out{keys, 8, dists, 4, nullptr, computed_out, visited_out};
+    return search_round_trip(q, nq, stride, query_scalar, 1, out, &total, [&](void const* dq, size_t vs, device_results_t const& r) {
+        return search_device(dq, nq, vs, 1, r.keys, r.dists, r.counts, r.computed, r.visited, stream, false, filter);
+    });
 }
 
 /* One query per call, many calling threads: gather what is waiting into one batch. The first caller to find no leader
@@ -809,8 +809,7 @@ char const* frozen_index_t::search_single(void const* query, uint32_t query_scal
         char const* e = nullptr;
         if (nq == 1) {
             size_t total = 0;
-            e = search_host(batch[0]->query, 1, 0, batch[0]->scalar, k, batch[0]->keys, k * 8, batch[0]->dists, k * 4, nullptr, nullptr,
-                            nullptr, &total);
+            e = search_host(batch[0]->query, 1, 0, batch[0]->scalar, k, host_results_t{batch[0]->keys, k * 8, batch[0]->dists, k * 4}, &total);
             batch[0]->found = total;
         } else {
             std::vector<uint8_t> q(nq * qbytes);
@@ -818,8 +817,9 @@ char const* frozen_index_t::search_single(void const* query, uint32_t query_scal
             std::vector<float> out_d(nq * k);
             std::vector<size_t> cnt(nq);
             for (size_t i = 0; i < nq; ++i) std::memcpy(q.data() + i * qbytes, batch[i]->query, qbytes);
-            e = search_host(q.data(), nq, qbytes, batch[0]->scalar, k, out_k.data(), k * 8, out_d.data(), k * 4, cnt.data(), nullptr,
-                            nullptr, nullptr);
+            size_t total = 0;
+            e = search_host(q.data(), nq, qbytes, batch[0]->scalar, k, host_results_t{out_k.data(), k * 8, out_d.data(), k * 4, cnt.data()},
+                            &total);
             for (size_t i = 0; i < nq && !e; ++i) {
                 std::memcpy(batch[i]->keys, out_k.data() + i * k, k * 8);
                 std::memcpy(batch[i]->dists, out_d.data() + i * k, k * 4);
@@ -843,35 +843,18 @@ char const* frozen_index_t::search_single(void const* query, uint32_t query_scal
 /* ---------------------------------------------------------------------------------------------- */
 
 /* index_gt::search(exact = true) (index.hpp:3047-3051 -> search_exact_ :4251-4268) for a batch of host queries */
-char const* frozen_index_t::exact_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t* keys,
-                                       float* dists, size_t* counts_out) {
+char const* frozen_index_t::exact_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k, host_results_t const& out,
+                                       size_t* total) {
     if (nq == 0 || k == 0) return nullptr;
     std::lock_guard<std::mutex> lock(mutex);
-    if (!loaded || d.n == 0) {
-        for (size_t i = 0; i < nq; ++i) {
-            for (size_t j = 0; j < k; ++j) { keys[i * k + j] = 0; reinterpret_cast<uint32_t*>(dists)[i * k + j] = SNAN_BITS; }
-            if (counts_out) counts_out[i] = 0;
-        }
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
+                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
+        if (char const* e = exact_search_device(d, stream.sm_count, dq, nq, vs, k, false, false, r.keys, r.dists, r.counts, exact_scratch, stream))
+            return e;
+        kernel_launches += 2;
         return nullptr;
-    }
-    if (char const* e = ensure_context()) return e;
-    size_t const vs = d.vec_stride ? d.vec_stride : 16;
-    if (char const* e = queries.reserve(nq * vs)) return e;
-    if (char const* e = out_keys.reserve(nq * k)) return e;
-    if (char const* e = out_dists.reserve(nq * k)) return e;
-    if (char const* e = counts_reserve_all(nq)) return e;
-    if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
-    if (char const* e = exact_search_device(d, stream.sm_count, queries.ptr, nq, vs, k, false, false, out_keys.ptr, out_dists.ptr, counts.ptr,
-                                            exact_scratch, stream))
-        return e;
-    kernel_launches += 2;
-    CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_counts.ptr, counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));
-    if (counts_out)
-        for (size_t i = 0; i < nq; ++i) counts_out[i] = h_counts.ptr[i];
-    return nullptr;
+    });
 }
 
 /* usearch_distance: both vectors to the device, one warp, the metric struct of the search kernels */

@@ -11,6 +11,7 @@
 #include <cstdint>
 #include <condition_variable>
 #include <deque>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -79,6 +80,37 @@ struct build_scratch_t {
 
 struct shard_group_t; /* shards.cu */
 
+/* what search_device filters by: a bitmap over slots (filtered search), the last level of the greedy descent (cluster) */
+struct search_filter_t {
+    uint32_t const* allow_bits = nullptr;
+    int cluster_end_level = -1;
+};
+
+/* the host outputs of one search batch: rows of k keys / distances `keys_stride` / `dists_stride` bytes apart; counts,
+ * computed and visited (one per query) may be NULL */
+struct host_results_t {
+    uint64_t* keys;
+    size_t keys_stride;
+    float* dists;
+    size_t dists_stride;
+    size_t* counts = nullptr;
+    uint64_t* computed = nullptr;
+    uint64_t* visited = nullptr;
+};
+/* the dense device outputs search_round_trip hands its device call; computed / visited are NULL unless the host caller
+ * asked for them */
+struct device_results_t {
+    uint64_t* keys;
+    float* dists;
+    uint32_t* counts;
+    uint32_t* computed;
+    uint32_t* visited;
+};
+/* the device call of a host search: queries in the index's kind, rows `stride` bytes apart, outputs in `out` */
+using device_search_t = std::function<char const*(void const* d_queries, size_t stride, device_results_t const& out)>;
+/* index_gt::search on an empty index: no matches, no error (index.hpp:3036-3037); every row key 0 and a signalling NaN */
+char const* answer_empty(size_t nq, size_t k, host_results_t const& out);
+
 struct frozen_index_t {
     /* configuration (usearch_init_options_t) */
     uint32_t metric = 0, scalar = 0; /* reference char codes */
@@ -145,8 +177,7 @@ struct frozen_index_t {
     device_buffer_t<uint8_t> queries;
     device_buffer_t<uint64_t> allowed_keys; /* filtered search: sorted allowed keys and the bitmap built from them */
     device_buffer_t<uint32_t> allow_bits;
-    uint32_t const* active_allow_bits = nullptr; /* set for the duration of one filtered call */
-    int active_cluster_end_level = -1;           /* set for the duration of one cluster() call */
+    device_buffer_t<uint64_t> key_stage; /* the keys of a host entry (allowed keys, set keys), uploaded as given */
     device_buffer_t<uint64_t> out_keys;
     device_buffer_t<float> out_dists;
     pinned_buffer_t<uint8_t> h_queries;
@@ -210,8 +241,8 @@ struct frozen_index_t {
     void leave_shards();
     char const* sharded_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t* d_keys, float* d_dists,
                                       uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles, cudaStream_t stream);
-    char const* sharded_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t* keys,
-                                    float* dists, size_t* counts);
+    char const* sharded_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                    host_results_t const& out, size_t* total);
 
     /* device_keys.cu: lookups by key from device memory, through a key -> slot table in HBM built on first use */
     struct key_table_t {
@@ -227,6 +258,8 @@ struct frozen_index_t {
     char const* filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t const* allowed,
                                        size_t allowed_count, uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed,
                                        uint32_t* d_visited, cudaStream_t s);
+    char const* filtered_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t const* allowed,
+                                     size_t allowed_count, host_results_t const& out, size_t* total);
 
     /* grouped_filter.cu: a batch whose query i is filtered by key set groups[i], the sets given as CSR (offsets[G + 1] into
      * set_keys), every pointer in device memory. One bitmap row per set, built from the key table; rows of as many sets
@@ -234,7 +267,7 @@ struct frozen_index_t {
     device_buffer_t<uint32_t> group_bits; /* the rows of one round; counted by memory_usage */
     device_buffer_t<uint32_t> group_order, group_sorted, group_ids, group_bounds, group_flag;
     device_buffer_t<uint8_t> group_sort_temp;
-    device_buffer_t<uint64_t> group_offsets; /* the host entry's upload of `offsets` (its keys go to `allowed_keys`) */
+    device_buffer_t<uint64_t> group_offsets; /* a host entry's upload of `offsets` (its keys go to `key_stage`) */
     device_buffer_t<uint32_t> group_upload;   /* ... and of `groups` */
     char const* grouped_filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
                                                uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
@@ -242,7 +275,7 @@ struct frozen_index_t {
                                                cudaStream_t s);
     char const* grouped_filtered_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
                                              uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                             uint64_t* keys, float* dists, size_t* counts, uint64_t* computed, uint64_t* visited);
+                                             host_results_t const& out, size_t* total);
 
     /* grouped_filter.cu, exact form: search_exact_ over the live slots of each query's set (LISTED exact kernels). `groups`
      * may be NULL when group_count == 1. The scratch is counted by memory_usage and freed by clear. */
@@ -259,7 +292,7 @@ struct frozen_index_t {
                                             float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited, cudaStream_t s);
     char const* grouped_exact_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
                                           uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                          uint64_t* keys, float* dists, size_t* counts, uint64_t* computed);
+                                          host_results_t const& out, size_t* total);
 
     /* searches */
     /* grouped: plan for the GROUPED kernel (its occupancy) */
@@ -267,7 +300,8 @@ struct frozen_index_t {
                      bool grouped = false) const;
     char const* prepare_launch(launch_plan_t const& pl, size_t warps, search_args_t& a, cudaStream_t s);
     char const* search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint64_t* d_keys, float* d_dists,
-                              uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles, cudaStream_t stream, bool defer = false);
+                              uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_cycles, cudaStream_t stream, bool defer = false,
+                              search_filter_t const& filter = {});
     /* deferred launches (usearch_b200_search_many_enqueue): status words and arguments kept until search_finish */
     struct pending_search_t { uint32_t* status; search_args_t args; bool maxed; cudaStream_t stream; };
     std::vector<pending_search_t> pending;
@@ -287,13 +321,18 @@ struct frozen_index_t {
     uint64_t gathered_batches = 0, gathered_queries = 0;
     char const* search_single(void const* query, uint32_t query_scalar, size_t count, uint64_t* keys, float* dists, size_t* found);
     char const* upload_queries(void const* queries, size_t nq, size_t stride, uint32_t query_scalar);
+    char const* stage_keys(uint64_t const* keys, size_t n);
+    /* every host search entry, once it has its lock and its checks passed on a non-empty index: the queries up, `search`
+     * on the device, the rows down into `out`; *total = the sum of counts */
+    char const* search_round_trip(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                  host_results_t const& out, size_t* total, device_search_t const& search);
     device_buffer_t<uint8_t> exact_scratch;
-    char const* exact_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t* keys,
-                           float* dists, size_t* counts);
-    char const* search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t* keys,
-                            size_t keys_stride, float* dists, size_t dists_stride, size_t* counts, uint64_t* computed,
-                            uint64_t* cycles, size_t* total, uint64_t const* allowed = nullptr, size_t allowed_count = 0,
-                            bool filtered = false, int cluster_level = -1);
+    char const* exact_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, host_results_t const& out,
+                           size_t* total);
+    char const* search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, host_results_t const& out,
+                            size_t* total);
+    char const* cluster_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t level, uint64_t* keys,
+                             float* dists, uint64_t* computed, uint64_t* visited);
 };
 
 /* exact_kernel.cu */

@@ -47,6 +47,62 @@ __global__ void grouped_validate_kernel(uint32_t const* groups, size_t nq, uint6
     }
 }
 
+/* what each grouped entry accepts beyond the CSR rules both share */
+struct key_set_rules_t {
+    uint64_t max_sets;    /* refused from this many sets on */
+    bool groups_optional; /* `groups` may be NULL when there is one set: every query uses set 0 */
+    uint64_t max_entries; /* keys in all the sets */
+};
+constexpr key_set_rules_t GRAPH_SETS{0xFFFFFFFFull, false, UINT64_MAX};
+constexpr key_set_rules_t EXACT_SETS{0x7FFFFFFFull, true, 0x7FFFFFFFull};
+
+/* the sets of a host entry, checked before anything is uploaded (the offsets size the upload) */
+char const* check_key_sets_host(uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count, key_set_rules_t const& rules) {
+    if (group_count == 0) return ERR_NO_SETS;
+    if (!groups && !(rules.groups_optional && group_count == 1)) return ERR_NO_GROUPS;
+    if (offsets[0] != 0) return ERR_OFFSETS;
+    for (size_t g = 0; g < group_count; ++g)
+        if (offsets[g + 1] < offsets[g]) return ERR_OFFSETS;
+    if (groups)
+        for (size_t i = 0; i < nq; ++i)
+            if (groups[i] >= group_count) return ERR_GROUP;
+    return nullptr;
+}
+
+/* the sets of a device entry, checked on the device before any output is written: one launch, one read-back, which also
+ * brings back the number of keys in all the sets */
+char const* check_key_sets_device(frozen_index_t& ix, uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count,
+                                  key_set_rules_t const& rules, uint64_t* entries, cudaStream_t s) {
+    if (group_count == 0) return ERR_NO_SETS;
+    if (group_count >= rules.max_sets) return "Too many key sets in one call";
+    if (!groups && !(rules.groups_optional && group_count == 1)) return ERR_NO_GROUPS;
+    if (char const* e = ix.group_flag.reserve(1)) return e;
+    CU(cudaMemsetAsync(ix.group_flag.ptr, 0, 4, s));
+    grouped_validate_kernel<<<grid_for(std::max(nq, group_count), ix.stream.sm_count), 256, 0, s>>>(groups, groups ? nq : 0, offsets,
+                                                                                                    group_count, ix.group_flag.ptr);
+    CU(cudaGetLastError());
+    ix.kernel_launches += 1;
+    uint32_t flag = 0;
+    CU(cudaMemcpyAsync(&flag, ix.group_flag.ptr, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(entries, offsets + group_count, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (flag & BAD_GROUP) return ERR_GROUP;
+    if (flag & BAD_OFFSETS) return ERR_OFFSETS;
+    if (*entries > rules.max_entries) return "Too many keys in one call's sets";
+    return nullptr;
+}
+
+/* a host entry's sets to the device: `groups` (when given) to group_upload, `offsets` to group_offsets, the keys to key_stage */
+char const* upload_key_sets(frozen_index_t& ix, uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count,
+                            uint64_t const* set_keys) {
+    if (char const* e = ix.group_upload.reserve(nq)) return e;
+    if (char const* e = ix.group_offsets.reserve(group_count + 1)) return e;
+    if (char const* e = ix.stage_keys(set_keys, offsets[group_count])) return e;
+    if (groups) CU(cudaMemcpyAsync(ix.group_upload.ptr, groups, nq * 4, cudaMemcpyHostToDevice, ix.stream));
+    CU(cudaMemcpyAsync(ix.group_offsets.ptr, offsets, (group_count + 1) * 8, cudaMemcpyHostToDevice, ix.stream));
+    return nullptr;
+}
+
 /* rows[(g - g0) * words ..] |= the slots of every key of set g, for g0 <= g < g1; the rows start zeroed. The free key
  * allows the removed slots, as allow_bits_kernel's search of keys[] does (the deleted bits reject them first anyway). */
 __global__ void grouped_bits_kernel(key_cell_t const* cells, uint64_t mask, uint64_t const* offsets, uint64_t const* set_keys, uint32_t g0,
@@ -210,21 +266,8 @@ char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries
     if (char const* e = ensure_context()) return e;
     if (nq == 0 || k == 0) return nullptr;
     if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
-    if (group_count == 0) return ERR_NO_SETS;
-    if (group_count >= 0xFFFFFFFFull) return "Too many key sets in one call";
-
-    /* every refusal comes before the first write to an output */
-    if (char const* e = group_flag.reserve(1)) return e;
-    CU(cudaMemsetAsync(group_flag.ptr, 0, 4, s));
-    grouped_validate_kernel<<<grid_for(std::max(nq, group_count), stream.sm_count), 256, 0, s>>>(groups, nq, offsets, group_count,
-                                                                                                 group_flag.ptr);
-    CU(cudaGetLastError());
-    kernel_launches += 1;
-    uint32_t flag = 0;
-    CU(cudaMemcpyAsync(&flag, group_flag.ptr, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    if (flag & BAD_GROUP) return ERR_GROUP;
-    if (flag & BAD_OFFSETS) return ERR_OFFSETS;
+    uint64_t entries = 0;
+    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, GRAPH_SETS, &entries, s)) return e;
 
     if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
         CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
@@ -317,59 +360,21 @@ char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries
     return nullptr;
 }
 
-/* host queries of any kind, host sets and host outputs: validated here (the offsets size the upload), uploaded, and run
- * through the device path */
+/* host queries of any kind, host sets and host outputs: the sets checked here, then uploaded and run through the device path */
 char const* frozen_index_t::grouped_filtered_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
                                                          uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                         uint64_t const* set_keys, uint64_t* keys, float* dists, size_t* counts_out,
-                                                         uint64_t* computed_out, uint64_t* visited_out) {
+                                                         uint64_t const* set_keys, host_results_t const& out, size_t* total) {
     std::lock_guard<std::mutex> lock(mutex);
     if (shards) return ERR_SHARDED;
     if (nq == 0 || k == 0) return nullptr;
-    if (group_count == 0) return ERR_NO_SETS;
-    if (offsets[0] != 0) return ERR_OFFSETS;
-    for (size_t g = 0; g < group_count; ++g)
-        if (offsets[g + 1] < offsets[g]) return ERR_OFFSETS;
-    for (size_t i = 0; i < nq; ++i)
-        if (groups[i] >= group_count) return ERR_GROUP;
-    if (!loaded || d.n == 0) { /* as search_host answers on an empty index */
-        for (size_t i = 0; i < nq; ++i) {
-            for (size_t j = 0; j < k; ++j) { keys[i * k + j] = 0; reinterpret_cast<uint32_t*>(dists)[i * k + j] = SNAN_BITS; }
-            if (counts_out) counts_out[i] = 0;
-            if (computed_out) computed_out[i] = 0;
-            if (visited_out) visited_out[i] = 0;
-        }
-        return nullptr;
-    }
-    if (char const* e = ensure_context()) return e;
-    size_t const vs = d.vec_stride ? d.vec_stride : 16, total = offsets[group_count];
-    if (char const* e = queries.reserve(nq * vs)) return e;
-    if (char const* e = out_keys.reserve(nq * k)) return e;
-    if (char const* e = out_dists.reserve(nq * k)) return e;
-    if (char const* e = counts_reserve_all(nq)) return e;
-    if (char const* e = group_upload.reserve(nq)) return e;
-    if (char const* e = group_offsets.reserve(group_count + 1)) return e;
-    if (char const* e = allowed_keys.reserve(std::max<size_t>(total, 1))) return e;
-    if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
-    CU(cudaMemcpyAsync(group_upload.ptr, groups, nq * 4, cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(group_offsets.ptr, offsets, (group_count + 1) * 8, cudaMemcpyHostToDevice, stream));
-    if (total) CU(cudaMemcpyAsync(allowed_keys.ptr, set_keys, total * 8, cudaMemcpyHostToDevice, stream));
-    if (char const* e = grouped_filtered_search_device(queries.ptr, nq, vs, k, group_upload.ptr, group_offsets.ptr, group_count,
-                                                       allowed_keys.ptr, out_keys.ptr, out_dists.ptr, this->counts.ptr, computed.ptr,
-                                                       cycles.ptr, stream))
-        return e;
-    CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_counts.ptr, this->counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_computed.ptr, computed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_cycles.ptr, cycles.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));
-    for (size_t i = 0; i < nq; ++i) {
-        if (counts_out) counts_out[i] = h_counts.ptr[i];
-        if (computed_out) computed_out[i] = h_computed.ptr[i];
-        if (visited_out) visited_out[i] = h_cycles.ptr[i];
-    }
-    return nullptr;
+    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, GRAPH_SETS)) return e;
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
+                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
+        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
+        return grouped_filtered_search_device(dq, nq, vs, k, group_upload.ptr, group_offsets.ptr, group_count, key_stage.ptr, r.keys, r.dists,
+                                              r.counts, r.computed, r.visited, stream);
+    });
 }
 
 /* ---------------------------------------------------------------------------------------------- */
@@ -391,26 +396,9 @@ char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, s
     if (char const* e = ensure_context()) return e;
     if (nq == 0 || k == 0) return nullptr;
     if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
-    if (group_count == 0) return ERR_NO_SETS;
-    if (group_count >= 0x7FFFFFFFull) return "Too many key sets in one call";
-    if (!groups && group_count != 1) return ERR_NO_GROUPS;
-    exact_filter_scratch_t& x = exact_filter;
-
-    /* every refusal comes before the first write to an output: the flag and the entry count in one read-back */
-    if (char const* e = group_flag.reserve(1)) return e;
-    CU(cudaMemsetAsync(group_flag.ptr, 0, 4, s));
-    grouped_validate_kernel<<<grid_for(std::max(nq, group_count), stream.sm_count), 256, 0, s>>>(groups, groups ? nq : 0, offsets, group_count,
-                                                                                                 group_flag.ptr);
-    CU(cudaGetLastError());
-    kernel_launches += 1;
-    uint32_t flag = 0;
     uint64_t entries = 0;
-    CU(cudaMemcpyAsync(&flag, group_flag.ptr, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&entries, offsets + group_count, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    if (flag & BAD_GROUP) return ERR_GROUP;
-    if (flag & BAD_OFFSETS) return ERR_OFFSETS;
-    if (entries > 0x7FFFFFFFull) return "Too many keys in one call's sets";
+    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, EXACT_SETS, &entries, s)) return e;
+    exact_filter_scratch_t& x = exact_filter;
 
     if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
         CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
@@ -534,57 +522,21 @@ char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, s
     return nullptr;
 }
 
-/* host queries of any kind, host sets and host outputs: checked here (the offsets size the upload), uploaded, and run through
- * the device path, as grouped_filtered_search_host does */
+/* host queries of any kind, host sets and host outputs, as grouped_filtered_search_host serves them */
 char const* frozen_index_t::grouped_exact_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
                                                       uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                                      uint64_t* keys, float* dists, size_t* counts_out, uint64_t* computed_out) {
+                                                      host_results_t const& out, size_t* total) {
     std::lock_guard<std::mutex> lock(mutex);
     if (shards) return ERR_SHARDED;
     if (nq == 0 || k == 0) return nullptr;
-    if (group_count == 0) return ERR_NO_SETS;
-    if (!groups && group_count != 1) return ERR_NO_GROUPS;
-    if (offsets[0] != 0) return ERR_OFFSETS;
-    for (size_t g = 0; g < group_count; ++g)
-        if (offsets[g + 1] < offsets[g]) return ERR_OFFSETS;
-    if (groups)
-        for (size_t i = 0; i < nq; ++i)
-            if (groups[i] >= group_count) return ERR_GROUP;
-    if (!loaded || d.n == 0) { /* as exact_host answers on an empty index */
-        for (size_t i = 0; i < nq; ++i) {
-            for (size_t j = 0; j < k; ++j) { keys[i * k + j] = 0; reinterpret_cast<uint32_t*>(dists)[i * k + j] = SNAN_BITS; }
-            if (counts_out) counts_out[i] = 0;
-            if (computed_out) computed_out[i] = 0;
-        }
-        return nullptr;
-    }
-    if (char const* e = ensure_context()) return e;
-    size_t const vs = d.vec_stride ? d.vec_stride : 16, total = offsets[group_count];
-    if (char const* e = queries.reserve(nq * vs)) return e;
-    if (char const* e = out_keys.reserve(nq * k)) return e;
-    if (char const* e = out_dists.reserve(nq * k)) return e;
-    if (char const* e = counts_reserve_all(nq)) return e;
-    if (char const* e = group_upload.reserve(nq)) return e;
-    if (char const* e = group_offsets.reserve(group_count + 1)) return e;
-    if (char const* e = allowed_keys.reserve(std::max<size_t>(total, 1))) return e;
-    if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
-    if (groups) CU(cudaMemcpyAsync(group_upload.ptr, groups, nq * 4, cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(group_offsets.ptr, offsets, (group_count + 1) * 8, cudaMemcpyHostToDevice, stream));
-    if (total) CU(cudaMemcpyAsync(allowed_keys.ptr, set_keys, total * 8, cudaMemcpyHostToDevice, stream));
-    if (char const* e = grouped_exact_search_device(queries.ptr, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count,
-                                                    allowed_keys.ptr, out_keys.ptr, out_dists.ptr, this->counts.ptr, computed.ptr, nullptr,
-                                                    stream))
-        return e;
-    CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_counts.ptr, this->counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_computed.ptr, computed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));
-    for (size_t i = 0; i < nq; ++i) {
-        if (counts_out) counts_out[i] = h_counts.ptr[i];
-        if (computed_out) computed_out[i] = h_computed.ptr[i];
-    }
-    return nullptr;
+    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, EXACT_SETS)) return e;
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
+                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
+        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
+        return grouped_exact_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count, key_stage.ptr,
+                                           r.keys, r.dists, r.counts, r.computed, nullptr, stream);
+    });
 }
 
 } // namespace usearch_b200

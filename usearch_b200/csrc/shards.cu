@@ -189,29 +189,17 @@ char const* frozen_index_t::sharded_search_device(void const* d_queries, size_t 
 }
 
 /* the same on host buffers: H2D of the queries and D2H of the merged rows inside the call */
-char const* frozen_index_t::sharded_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t* keys,
-                                                float* dists, size_t* counts_out) {
+char const* frozen_index_t::sharded_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                host_results_t const& out, size_t* total) {
     if (nq == 0 || k == 0) return nullptr;
     std::lock_guard<std::mutex> lock(mutex);
     if (char const* e = ensure_context()) return e;
     if (!configured()) return "Index is not initialized";
     if (!loaded) /* an empty shard still takes part in the exchange */
         if (char const* e = reserve_slots(0)) return e;
-    size_t const vs = d.vec_stride ? d.vec_stride : 16;
-    if (char const* e = queries.reserve(nq * vs)) return e;
-    if (char const* e = out_keys.reserve(nq * k)) return e;
-    if (char const* e = out_dists.reserve(nq * k)) return e;
-    if (char const* e = counts_reserve_all(nq)) return e;
-    if (char const* e = upload_queries(q, nq, stride, query_scalar)) return e;
-    if (char const* e = sharded_search_device(queries.ptr, nq, vs, k, out_keys.ptr, out_dists.ptr, this->counts.ptr, nullptr, nullptr, stream))
-        return e;
-    CU(cudaMemcpyAsync(keys, out_keys.ptr, nq * k * 8, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(dists, out_dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_counts.ptr, this->counts.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));
-    if (counts_out)
-        for (size_t i = 0; i < nq; ++i) counts_out[i] = h_counts.ptr[i];
-    return nullptr;
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total, [&](void const* dq, size_t vs, device_results_t const& r) {
+        return sharded_search_device(dq, nq, vs, k, r.keys, r.dists, r.counts, r.computed, r.visited, stream);
+    });
 }
 
 /* `world` payloads (host memory, back to back, each shards_payload_bytes(nq, k) long) -> merged rows (host memory): the
