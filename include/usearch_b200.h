@@ -393,6 +393,45 @@ void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t inde
                                                             usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                                             uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error);
 
+/* Excluded search: the sets of usearch_b200_grouped_filtered_search_many name keys a query must NOT return. Row i equals
+ * the reference's filtered_search(queries[i], count, key not in set groups[i]) (index_dense.hpp:774-779): keys,
+ * distances, counts and both counters. A removed entry is never returned; a free key, a key the index lacks or a repeated
+ * key in a set changes nothing; on a multi index excluding a key excludes every entry under it; an empty set gives the
+ * plain search's row. `groups` may be NULL when sets_count is 1: every query uses set 0. Each set becomes a bitmap row
+ * that allows every slot but the set's, served in rounds under the "group_bitmap_mb" knob. Refusals as in
+ * usearch_b200_grouped_filtered_search_many, before any output is written. Buffers are HOST memory; queries may be of
+ * any kind. Returns the sum of counts. */
+size_t usearch_b200_grouped_excluded_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                 size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                 uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                 usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                 size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
+                                                 usearch_error_t* error);
+/* The same with DEVICE queries (in the index's kind), DEVICE groups, offsets, set keys and outputs, on `cuda_stream`
+ * (NULL = the handle's stream). The call returns when the outputs are complete. */
+void usearch_b200_grouped_excluded_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                      size_t queries_stride, size_t count, uint32_t const* groups,
+                                                      uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                      usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                      uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
+                                                      usearch_error_t* error);
+/* Exact excluded search: every query scans exactly the live entries whose key is not in its set, as the reference's
+ * filtered_search(..., exact = true) does (index.hpp:4251-4268): keys, distances and counts equal it, and
+ * computed_distances[i] = the live entries less the e live entries under the set's keys. It runs the unfiltered exact
+ * search at count k + e rounded up to a power of two (one launch per such count) and drops the set's entries, so
+ * k + e > 256 is refused, with exact search's message, for vectors too long for its tiled stage. Refusals and buffers as
+ * in usearch_b200_grouped_filtered_exact_search_many. */
+size_t usearch_b200_grouped_excluded_exact_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                       size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                       uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                       usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                       size_t* counts, uint64_t* computed_distances, usearch_error_t* error);
+void usearch_b200_grouped_excluded_exact_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                            size_t queries_stride, size_t count, uint32_t const* groups,
+                                                            uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                            usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                            uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error);
+
 /* The asynchronous pair. `enqueue` = the same arguments as usearch_b200_search_many_device, but it ONLY enqueues the
  * kernel on `cuda_stream` and returns; any number of batches may be in flight. `finish` waits for them, inspects the
  * per-query status words and re-runs, with larger scratch, the rare queries whose scratch overflowed; the outputs of

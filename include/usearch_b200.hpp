@@ -344,6 +344,52 @@ class index_dense_t {
                                                                cuda_stream, &e);
         return e;
     }
+    /* query i searches every live entry whose key is NOT in set groups[i] (usearch_b200_grouped_excluded_search_many);
+     * `groups` may be NULL with one set */
+    template <typename scalar_at>
+    error_t grouped_excluded_search(scalar_at const* queries, std::size_t queries_count, std::size_t queries_stride, std::size_t wanted,
+                                    std::uint32_t const* groups, std::uint64_t const* offsets, std::size_t sets_count,
+                                    vector_key_t const* set_keys, vector_key_t* keys, distance_t* distances, std::size_t* counts,
+                                    std::uint64_t* computed_distances = nullptr, std::uint64_t* visited_members = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_excluded_search_many(handle_, queries, queries_count, queries_stride, scalar_kind<scalar_at>(), wanted, groups, offsets,
+                                                  sets_count, set_keys, keys, distances, counts, computed_distances, visited_members, &e);
+        return e;
+    }
+    error_t grouped_excluded_search_device(void const* queries, std::size_t queries_count, std::size_t queries_stride, std::size_t wanted,
+                                           std::uint32_t const* groups, std::uint64_t const* offsets, std::size_t sets_count,
+                                           vector_key_t const* set_keys, vector_key_t* keys, distance_t* distances, std::uint32_t* counts,
+                                           std::uint32_t* computed_distances = nullptr, std::uint32_t* visited_members = nullptr,
+                                           void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_excluded_search_many_device(handle_, queries, queries_count, queries_stride, wanted, groups, offsets,
+                                                         sets_count, set_keys, keys, distances, counts, computed_distances,
+                                                         visited_members, cuda_stream, &e);
+        return e;
+    }
+    template <typename scalar_at>
+    error_t grouped_excluded_exact_search(scalar_at const* queries, std::size_t queries_count, std::size_t queries_stride,
+                                          std::size_t wanted, std::uint32_t const* groups, std::uint64_t const* offsets,
+                                          std::size_t sets_count, vector_key_t const* set_keys, vector_key_t* keys,
+                                          distance_t* distances, std::size_t* counts,
+                                          std::uint64_t* computed_distances = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_excluded_exact_search_many(handle_, queries, queries_count, queries_stride, scalar_kind<scalar_at>(), wanted,
+                                                        groups, offsets, sets_count, set_keys, keys, distances, counts,
+                                                        computed_distances, &e);
+        return e;
+    }
+    error_t grouped_excluded_exact_search_device(void const* queries, std::size_t queries_count, std::size_t queries_stride,
+                                                 std::size_t wanted, std::uint32_t const* groups, std::uint64_t const* offsets,
+                                                 std::size_t sets_count, vector_key_t const* set_keys, vector_key_t* keys,
+                                                 distance_t* distances, std::uint32_t* counts,
+                                                 std::uint32_t* computed_distances = nullptr, void* cuda_stream = nullptr) const {
+        usearch_error_t e = nullptr;
+        usearch_b200_grouped_excluded_exact_search_many_device(handle_, queries, queries_count, queries_stride, wanted, groups, offsets,
+                                                               sets_count, set_keys, keys, distances, counts, computed_distances,
+                                                               cuda_stream, &e);
+        return e;
+    }
     /* index_dense.hpp:774-779. `exact`: predicate(key) is called once per live entry on the host and the entries it accepts
      * are scanned on the device; otherwise the predicate goes to usearch_filtered_search, which cannot run a host callback
      * on the device and reports so. `thread` is accepted and ignored. */

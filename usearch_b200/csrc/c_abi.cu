@@ -438,6 +438,59 @@ void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t inde
     });
 }
 
+/* excluded search (grouped_filter.cu): query i searches the live entries whose key is not in set groups[i] */
+size_t usearch_b200_grouped_excluded_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                 size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                 uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                 usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                 size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
+                                                 usearch_error_t* error) {
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->grouped_excluded_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count,
+                                                             set_keys,
+                                                             host_results_t{keys, count * 8, distances, count * 4, counts,
+                                                                            computed_distances, visited_members},
+                                                             total);
+    });
+}
+
+void usearch_b200_grouped_excluded_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                      size_t queries_stride, size_t count, uint32_t const* groups,
+                                                      uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                      usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                      uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
+                                                      usearch_error_t* error) {
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
+        return ix->grouped_excluded_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
+                                                  keys, distances, counts, computed_distances, visited_members, s);
+    });
+}
+
+size_t usearch_b200_grouped_excluded_exact_search_many(usearch_index_t index, void const* queries, size_t queries_count,
+                                                       size_t queries_stride, usearch_scalar_kind_t query_kind, size_t count,
+                                                       uint32_t const* groups, uint64_t const* offsets, size_t sets_count,
+                                                       usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
+                                                       size_t* counts, uint64_t* computed_distances, usearch_error_t* error) {
+    return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
+        return as_index(index)->grouped_excluded_exact_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets,
+                                                                   sets_count, set_keys,
+                                                                   host_results_t{keys, count * 8, distances, count * 4, counts,
+                                                                                  computed_distances},
+                                                                   total);
+    });
+}
+
+void usearch_b200_grouped_excluded_exact_search_many_device(usearch_index_t index, void const* queries, size_t queries_count,
+                                                            size_t queries_stride, size_t count, uint32_t const* groups,
+                                                            uint64_t const* offsets, size_t sets_count, usearch_key_t const* set_keys,
+                                                            usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
+                                                            uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error) {
+    device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
+        return ix->grouped_excluded_exact_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
+                                                        keys, distances, counts, computed_distances, nullptr, s);
+    });
+}
+
 /* the asynchronous pair: enqueue any number of batches (kernel launches only, nothing waits), then finish once */
 void usearch_b200_search_many_enqueue(usearch_index_t index, void const* queries, size_t queries_count, size_t queries_stride,
                                       size_t count, usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,

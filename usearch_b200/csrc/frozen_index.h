@@ -276,11 +276,26 @@ struct frozen_index_t {
     char const* grouped_filtered_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
                                              uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
                                              host_results_t const& out, size_t* total);
+    /* excluded sets: query i searches the live entries whose key is NOT in set groups[i]; each row is the complement bitmap,
+     * all ones less the set's slots. `groups` may be NULL when group_count == 1. */
+    char const* grouped_excluded_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                               uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
+                                               float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                               cudaStream_t s);
+    char const* grouped_excluded_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                             uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
+                                             host_results_t const& out, size_t* total);
+    /* both graph forms: rows that allow the sets' slots, or (`excluded`) rows that allow every slot but them */
+    char const* grouped_rows_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                           uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, bool excluded,
+                                           uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                           cudaStream_t s);
 
     /* grouped_filter.cu, exact form: search_exact_ over the live slots of each query's set (LISTED exact kernels). `groups`
      * may be NULL when group_count == 1. The scratch is counted by memory_usage and freed by clear. */
     struct exact_filter_scratch_t {
         device_buffer_t<uint32_t> rows, list_at, query_at, per_set, item_at, order, sorted, ids, groups, scalars, counts;
+        device_buffer_t<uint32_t> buckets, bucket_at; /* the exact excluded search's buckets: per query, and their bounds */
         device_buffer_t<uint64_t> entry_counts, entry_at, words, words_sorted, keys;
         device_buffer_t<exact_item_t> items;
         device_buffer_t<uint8_t> temp, queries, exact;
@@ -293,6 +308,15 @@ struct frozen_index_t {
     char const* grouped_exact_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
                                           uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
                                           host_results_t const& out, size_t* total);
+    /* exact excluded search: search_exact_ over the live slots outside each query's set, as the unfiltered scan's top-(k + e)
+     * less the set's e live slots. Same scratch as the exact filtered form. */
+    char const* grouped_excluded_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                                     uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
+                                                     float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                                     cudaStream_t s);
+    char const* grouped_excluded_exact_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                   uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                   uint64_t const* set_keys, host_results_t const& out, size_t* total);
 
     /* searches */
     /* grouped: plan for the GROUPED kernel (its occupancy) */

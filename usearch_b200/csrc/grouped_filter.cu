@@ -12,6 +12,10 @@
  *  its live slots: one thread per entry counts the key's cells in the table, a scan places them, a second pass writes one
  *  (set << 32 | slot) word per cell, and a radix sort plus a unique leave the lists back to back. The queries, sorted by
  *  set and gathered, then run through the LISTED exact kernels, whose CTAs never mix sets (exact_kernel.cu).
+ *
+ *  Excluded sets (query i searches every live entry whose key is NOT in its set) reuse both: on the graph each row starts
+ *  all ones and loses the set's slots; the exact form runs the unfiltered scan at count k + e (e = the live slots of the
+ *  set, from its slot list) and drops the set's slots from each row.
  */
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -55,6 +59,7 @@ struct key_set_rules_t {
 };
 constexpr key_set_rules_t GRAPH_SETS{0xFFFFFFFFull, false, UINT64_MAX};
 constexpr key_set_rules_t EXACT_SETS{0x7FFFFFFFull, true, 0x7FFFFFFFull};
+constexpr key_set_rules_t EXCLUDED_GRAPH_SETS{0xFFFFFFFFull, true, UINT64_MAX};
 
 /* the sets of a host entry, checked before anything is uploaded (the offsets size the upload) */
 char const* check_key_sets_host(uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count, key_set_rules_t const& rules) {
@@ -128,6 +133,23 @@ __global__ void grouped_bits_kernel(key_cell_t const* cells, uint64_t mask, uint
             continue;
         }
         key_table_for_each(cells, mask, key, [&](uint32_t s) { atomicOr(row + (s >> 5), 1u << (s & 31)); });
+    }
+}
+
+/* excluded sets: rows[(g - g0) * words ..] &= ~(the slots of every key of set g); the rows start all ones. The table holds
+ * no cell of the free key, and the deleted bits reject removed slots before any row is read, so the free key needs no case. */
+__global__ void excluded_bits_kernel(key_cell_t const* cells, uint64_t mask, uint64_t const* offsets, uint64_t const* set_keys, uint32_t g0,
+                                     uint32_t g1, uint32_t words, uint32_t* rows) {
+    uint64_t const begin = offsets[g0], end = offsets[g1];
+    for (uint64_t e = begin + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < end; e += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t lo = g0 + 1, hi = g1; /* the first set past entry e: offsets[lo] > e */
+        while (lo < hi) {
+            uint32_t const mid = (lo + hi) >> 1;
+            if (offsets[mid] > e) hi = mid;
+            else lo = mid + 1;
+        }
+        uint32_t* const row = rows + (size_t)(lo - 1 - g0) * words;
+        key_table_for_each(cells, mask, set_keys[e], [&](uint32_t s) { atomicAnd(row + (s >> 5), ~(1u << (s & 31))); });
     }
 }
 
@@ -255,6 +277,69 @@ __global__ void listed_scatter_kernel(uint32_t const* order, uint32_t const* sor
     }
 }
 
+/* ---- exact excluded search ---- */
+
+/* bucket[i] = the least b with 2^b >= min(k + e, cap), e = the live slots of query i's set: the count its scan runs at is
+ * min(2^b, cap) */
+__global__ void excluded_bucket_kernel(uint32_t const* groups, uint32_t const* list_at, uint32_t nq, uint64_t k, uint64_t cap, uint32_t* bucket) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += gridDim.x * blockDim.x) {
+        uint32_t const g = groups[i];
+        uint64_t const want = min(k + (list_at[g + 1] - list_at[g]), cap);
+        uint32_t b = 0;
+        while (b < 63 && (1ull << b) < want) ++b;
+        bucket[i] = b;
+    }
+}
+
+/* one warp per query of a bucket: row p of the unfiltered scan (`width` slots, ascending under the scan's order) keeps its
+ * first k slots that are not in the query's sorted excluded list, as keys, in caller row order[p]; the rest of the row is
+ * padded. computed_distances = the live entries less the excluded ones. */
+__global__ void excluded_drop_kernel(uint32_t const* order, uint32_t const* groups, uint32_t const* list_at, uint32_t const* rows, uint32_t nq,
+                                     uint32_t width, uint32_t k, uint64_t const* slots, float const* dists, uint32_t const* counts,
+                                     uint64_t const* keys, uint32_t live, uint64_t* out_keys, float* out_dists, uint32_t* out_counts,
+                                     uint32_t* out_computed, uint32_t* out_visited) {
+    uint32_t const p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    uint32_t const lane = threadIdx.x & 31;
+    if (p >= nq) return;
+    uint32_t const i = order[p], g = groups[i];
+    uint32_t const* const list = rows + list_at[g];
+    uint32_t const e = list_at[g + 1] - list_at[g], n = counts[p];
+    uint32_t* const out_bits = reinterpret_cast<uint32_t*>(out_dists) + (size_t)i * k;
+    uint32_t kept = 0;
+    for (uint32_t j0 = 0; j0 < n && kept < k; j0 += 32) {
+        uint32_t const j = j0 + lane;
+        uint32_t slot = 0;
+        bool keep = false;
+        if (j < n) {
+            slot = (uint32_t)slots[(size_t)p * width + j];
+            uint32_t lo = 0, hi = e;
+            while (lo < hi) {
+                uint32_t const mid = (lo + hi) >> 1;
+                if (list[mid] < slot) lo = mid + 1;
+                else hi = mid;
+            }
+            keep = lo == e || list[lo] != slot;
+        }
+        uint32_t const ballot = __ballot_sync(0xFFFFFFFFu, keep);
+        uint32_t const at = kept + __popc(ballot & ((1u << lane) - 1u));
+        if (keep && at < k) {
+            out_keys[(size_t)i * k + at] = keys[slot];
+            out_bits[at] = reinterpret_cast<uint32_t const*>(dists)[(size_t)p * width + j];
+        }
+        kept += __popc(ballot);
+    }
+    kept = min(kept, k);
+    for (uint32_t j = kept + lane; j < k; j += 32) {
+        out_keys[(size_t)i * k + j] = 0;
+        out_bits[j] = SNAN_BITS;
+    }
+    if (lane == 0) {
+        out_counts[i] = kept;
+        if (out_computed) out_computed[i] = live - e;
+        if (out_visited) out_visited[i] = 0;
+    }
+}
+
 } // namespace
 
 char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
@@ -262,17 +347,40 @@ char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries
                                                            uint64_t const* set_keys, uint64_t* d_keys, float* d_dists,
                                                            uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
                                                            cudaStream_t s) {
+    return grouped_rows_search_device(d_queries, nq, stride, k, groups, offsets, group_count, set_keys, false, d_keys, d_dists, d_counts,
+                                      d_computed, d_visited, s);
+}
+
+char const* frozen_index_t::grouped_excluded_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
+                                                           uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                           uint64_t const* set_keys, uint64_t* d_keys, float* d_dists,
+                                                           uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
+                                                           cudaStream_t s) {
+    return grouped_rows_search_device(d_queries, nq, stride, k, groups, offsets, group_count, set_keys, true, d_keys, d_dists, d_counts,
+                                      d_computed, d_visited, s);
+}
+
+char const* frozen_index_t::grouped_rows_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
+                                                       uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, bool excluded,
+                                                       uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed,
+                                                       uint32_t* d_visited, cudaStream_t s) {
     if (shards) return ERR_SHARDED;
     if (char const* e = ensure_context()) return e;
     if (nq == 0 || k == 0) return nullptr;
     if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
     uint64_t entries = 0;
-    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, GRAPH_SETS, &entries, s)) return e;
+    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, excluded ? EXCLUDED_GRAPH_SETS : GRAPH_SETS, &entries, s))
+        return e;
 
     if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
         CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
         CU(cudaStreamSynchronize(s));
         return nullptr;
+    }
+    if (!groups) { /* one set: every query tests row 0 of the GROUPED kernel */
+        if (char const* e = group_upload.reserve(nq)) return e;
+        CU(cudaMemsetAsync(group_upload.ptr, 0, nq * 4, s));
+        groups = group_upload.ptr;
     }
     if (char const* e = ensure_key_table(s)) return e;
     uint32_t const words = (uint32_t)((size + 31) / 32);
@@ -293,9 +401,14 @@ char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries
 
     /* the sets [g0, g1) into rows, then their queries: `items` work items, through `list` when it is not NULL */
     auto round = [&](uint32_t g0, uint32_t g1, uint32_t const* list, size_t items) -> char const* {
-        CU(cudaMemsetAsync(group_bits.ptr, 0, (size_t)(g1 - g0) * words * 4, s));
-        grouped_bits_kernel<<<stream.sm_count * 16, 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, set_keys, g0, g1,
-                                                                 free_key, d.deleted_bits, (uint32_t)size, words, group_bits.ptr);
+        /* allowed sets: rows of zeros that gain their slots; excluded sets: rows of ones that lose theirs */
+        CU(cudaMemsetAsync(group_bits.ptr, excluded ? 0xFF : 0, (size_t)(g1 - g0) * words * 4, s));
+        if (excluded)
+            excluded_bits_kernel<<<stream.sm_count * 16, 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, set_keys, g0, g1, words,
+                                                                      group_bits.ptr);
+        else
+            grouped_bits_kernel<<<stream.sm_count * 16, 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, set_keys, g0, g1,
+                                                                     free_key, d.deleted_bits, (uint32_t)size, words, group_bits.ptr);
         CU(cudaGetLastError());
         kernel_launches += 1;
         int const blocks = (int)std::min<size_t>((size_t)pl.blocks, (items + wpb - 1) / wpb);
@@ -377,6 +490,23 @@ char const* frozen_index_t::grouped_filtered_search_host(void const* q, size_t n
     });
 }
 
+/* the same for excluded sets; `groups` may be NULL with one set */
+char const* frozen_index_t::grouped_excluded_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                         uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                         uint64_t const* set_keys, host_results_t const& out, size_t* total) {
+    std::lock_guard<std::mutex> lock(mutex);
+    if (shards) return ERR_SHARDED;
+    if (nq == 0 || k == 0) return nullptr;
+    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, EXCLUDED_GRAPH_SETS)) return e;
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
+                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
+        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
+        return grouped_excluded_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count, key_stage.ptr,
+                                              r.keys, r.dists, r.counts, r.computed, r.visited, stream);
+    });
+}
+
 /* ---------------------------------------------------------------------------------------------- */
 /*  exact filtered search: search_exact_ over the live slots of each query's key set              */
 /* ---------------------------------------------------------------------------------------------- */
@@ -385,8 +515,65 @@ size_t frozen_index_t::exact_filter_scratch_t::bytes() const {
     return entry_counts.capacity * 8 + entry_at.capacity * 8 + words.capacity * 8 + words_sorted.capacity * 8 + rows.capacity * 4 +
            list_at.capacity * 4 + query_at.capacity * 4 + per_set.capacity * 4 + item_at.capacity * 4 + items.capacity * sizeof(exact_item_t) +
            order.capacity * 4 + sorted.capacity * 4 + ids.capacity * 4 + groups.capacity * 4 + scalars.capacity * 4 + temp.capacity +
+           buckets.capacity * 4 + bucket_at.capacity * 4 +
            queries.capacity + keys.capacity * 8 + dists.capacity * 4 + counts.capacity * 4 + exact.capacity;
 }
+
+namespace {
+
+/* the slot-list build, step 1: the live slots of every entry, placed by an exclusive scan into x.entry_at (one extra zero
+ * count: its place, entry_at[n_entries], is the cell total). Nothing waits. */
+char const* listed_place_cells(frozen_index_t& ix, uint64_t const* set_keys, size_t n_entries, cudaStream_t s) {
+    frozen_index_t::exact_filter_scratch_t& x = ix.exact_filter;
+    size_t temp_bytes = 0;
+    if (char const* e = x.entry_counts.reserve(n_entries + 1)) return e;
+    if (char const* e = x.entry_at.reserve(n_entries + 1)) return e;
+    if (char const* e = x.scalars.reserve(4)) return e;
+    CU(cudaMemsetAsync(x.entry_counts.ptr + n_entries, 0, 8, s));
+    if (n_entries)
+        listed_count_kernel<<<grid_for(n_entries, ix.stream.sm_count), 256, 0, s>>>(ix.key_table.cells.ptr, ix.key_table.mask, set_keys,
+                                                                                    n_entries, x.entry_counts.ptr);
+    CU(cudaGetLastError());
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp_bytes, x.entry_counts.ptr, x.entry_at.ptr, (int)(n_entries + 1), s));
+    if (char const* e = x.temp.reserve(std::max<size_t>(temp_bytes, 1))) return e;
+    CU(cub::DeviceScan::ExclusiveSum(x.temp.ptr, temp_bytes, x.entry_counts.ptr, x.entry_at.ptr, (int)(n_entries + 1), s));
+    return nullptr;
+}
+
+/* the slot-list build, step 2, once the host knows the cell total (at most INT_MAX): (set << 32 | slot) words, sorted over
+ * the bits in use and deduplicated, leave set g's ascending, duplicate-free slots at x.rows[x.list_at[g] .. x.list_at[g + 1]) */
+char const* listed_build_lists(frozen_index_t& ix, uint64_t const* offsets, uint32_t sets, uint64_t const* set_keys, size_t n_entries,
+                               uint64_t cells, cudaStream_t s) {
+    frozen_index_t::exact_filter_scratch_t& x = ix.exact_filter;
+    auto temp_for = [&](size_t bytes) { return x.temp.reserve(std::max<size_t>(bytes, 1)); };
+    size_t temp_bytes = 0;
+    int const n_cells = (int)cells;
+    int end_bit = 32;
+    while (end_bit < 64 && ((uint64_t)(sets - 1) >> (end_bit - 32))) ++end_bit;
+    if (char const* e = x.words.reserve(std::max<size_t>(cells, 1))) return e;
+    if (char const* e = x.words_sorted.reserve(std::max<size_t>(cells, 1))) return e;
+    if (char const* e = x.rows.reserve(std::max<size_t>(cells, 1))) return e;
+    if (char const* e = x.list_at.reserve((size_t)sets + 1)) return e;
+    CU(cudaMemsetAsync(x.scalars.ptr, 0, 16, s));
+    if (n_cells) {
+        listed_write_kernel<<<grid_for(n_entries, ix.stream.sm_count), 256, 0, s>>>(ix.key_table.cells.ptr, ix.key_table.mask, offsets, sets,
+                                                                                    set_keys, n_entries, x.entry_at.ptr, x.words.ptr);
+        CU(cudaGetLastError());
+        CU(cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, x.words.ptr, x.words_sorted.ptr, n_cells, 0, end_bit, s));
+        if (char const* e = temp_for(temp_bytes)) return e;
+        CU(cub::DeviceRadixSort::SortKeys(x.temp.ptr, temp_bytes, x.words.ptr, x.words_sorted.ptr, n_cells, 0, end_bit, s));
+        CU(cub::DeviceSelect::Unique(nullptr, temp_bytes, x.words_sorted.ptr, x.words.ptr, x.scalars.ptr, n_cells, s));
+        if (char const* e = temp_for(temp_bytes)) return e;
+        CU(cub::DeviceSelect::Unique(x.temp.ptr, temp_bytes, x.words_sorted.ptr, x.words.ptr, x.scalars.ptr, n_cells, s));
+        ix.kernel_launches += 3;
+    }
+    listed_rows_kernel<<<grid_for(std::max<size_t>(cells, (size_t)sets + 1), ix.stream.sm_count), 256, 0, s>>>(
+        x.words.ptr, x.scalars.ptr, (uint32_t)cells, sets, x.rows.ptr, x.list_at.ptr);
+    CU(cudaGetLastError());
+    return nullptr;
+}
+
+} // namespace
 
 char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
                                                         uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
@@ -413,18 +600,8 @@ char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, s
     auto temp_for = [&](size_t bytes) { return x.temp.reserve(std::max<size_t>(bytes, 1)); };
     size_t temp_bytes = 0;
 
-    /* 1. the live slots of every entry, placed by an exclusive scan (one extra zero count: its place is the total) */
-    if (char const* e = x.entry_counts.reserve(n_entries + 1)) return e;
-    if (char const* e = x.entry_at.reserve(n_entries + 1)) return e;
-    if (char const* e = x.scalars.reserve(4)) return e;
-    CU(cudaMemsetAsync(x.entry_counts.ptr + n_entries, 0, 8, s));
-    if (n_entries)
-        listed_count_kernel<<<grid_for(n_entries, stream.sm_count), 256, 0, s>>>(key_table.cells.ptr, key_table.mask, set_keys, n_entries,
-                                                                                 x.entry_counts.ptr);
-    CU(cudaGetLastError());
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp_bytes, x.entry_counts.ptr, x.entry_at.ptr, (int)(n_entries + 1), s));
-    if (char const* e = temp_for(temp_bytes)) return e;
-    CU(cub::DeviceScan::ExclusiveSum(x.temp.ptr, temp_bytes, x.entry_counts.ptr, x.entry_at.ptr, (int)(n_entries + 1), s));
+    /* 1. the live slots of every entry, placed by an exclusive scan */
+    if (char const* e = listed_place_cells(*this, set_keys, n_entries, s)) return e;
     /* 2. the queries sorted by set, cut into work items of at most qpc queries that never mix sets (counted here, written
      * once the lists are placed) */
     if (char const* e = x.groups.reserve(nq)) return e;
@@ -463,29 +640,7 @@ char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, s
     if (cells > 0x7FFFFFFFull) return "Too many listed rows in one call";
 
     /* 3. (set << 32 | slot) words, sorted over the bits in use and deduplicated: per-set ascending slot lists */
-    int const n_cells = (int)cells;
-    int end_bit = 32;
-    while (end_bit < 64 && ((uint64_t)(sets - 1) >> (end_bit - 32))) ++end_bit;
-    if (char const* e = x.words.reserve(std::max<size_t>(cells, 1))) return e;
-    if (char const* e = x.words_sorted.reserve(std::max<size_t>(cells, 1))) return e;
-    if (char const* e = x.rows.reserve(std::max<size_t>(cells, 1))) return e;
-    if (char const* e = x.list_at.reserve(group_count + 1)) return e;
-    CU(cudaMemsetAsync(x.scalars.ptr, 0, 16, s));
-    if (n_cells) {
-        listed_write_kernel<<<grid_for(n_entries, stream.sm_count), 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, sets, set_keys,
-                                                                                 n_entries, x.entry_at.ptr, x.words.ptr);
-        CU(cudaGetLastError());
-        CU(cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, x.words.ptr, x.words_sorted.ptr, n_cells, 0, end_bit, s));
-        if (char const* e = temp_for(temp_bytes)) return e;
-        CU(cub::DeviceRadixSort::SortKeys(x.temp.ptr, temp_bytes, x.words.ptr, x.words_sorted.ptr, n_cells, 0, end_bit, s));
-        CU(cub::DeviceSelect::Unique(nullptr, temp_bytes, x.words_sorted.ptr, x.words.ptr, x.scalars.ptr, n_cells, s));
-        if (char const* e = temp_for(temp_bytes)) return e;
-        CU(cub::DeviceSelect::Unique(x.temp.ptr, temp_bytes, x.words_sorted.ptr, x.words.ptr, x.scalars.ptr, n_cells, s));
-        kernel_launches += 3;
-    }
-    listed_rows_kernel<<<grid_for(std::max<size_t>(cells, group_count + 1), stream.sm_count), 256, 0, s>>>(
-        x.words.ptr, x.scalars.ptr, (uint32_t)cells, sets, x.rows.ptr, x.list_at.ptr);
-    CU(cudaGetLastError());
+    if (char const* e = listed_build_lists(*this, offsets, sets, set_keys, n_entries, cells, s)) return e;
 
     listed_items_kernel<<<grid_for(group_count, stream.sm_count), 256, 0, s>>>(x.query_at.ptr, x.item_at.ptr, x.list_at.ptr, sets, qpc,
                                                                                x.items.ptr);
@@ -536,6 +691,131 @@ char const* frozen_index_t::grouped_exact_search_host(void const* q, size_t nq, 
         if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
         return grouped_exact_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count, key_stage.ptr,
                                            r.keys, r.dists, r.counts, r.computed, nullptr, stream);
+    });
+}
+
+/* ---------------------------------------------------------------------------------------------- */
+/*  exact excluded search: search_exact_ over the live slots outside each query's key set         */
+/* ---------------------------------------------------------------------------------------------- */
+
+/* The scan order (distance ascending, slot descending) is total, so the k best entries outside a set of e live slots are
+ * what remains of the unfiltered top-(k + e) once the set's slots are dropped. The sets become slot lists (the exact
+ * filtered search's build); the queries are bucketed by k + e rounded up to a power of two, and each bucket runs the
+ * unfiltered scan once at its count, with slots for keys, then the drop. */
+char const* frozen_index_t::grouped_excluded_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
+                                                                 uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                                 uint64_t const* set_keys, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
+                                                                 uint32_t* d_computed, uint32_t* d_visited, cudaStream_t s) {
+    if (shards) return ERR_SHARDED;
+    if (char const* e = ensure_context()) return e;
+    if (nq == 0 || k == 0) return nullptr;
+    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
+    uint64_t entries = 0;
+    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, EXACT_SETS, &entries, s)) return e;
+    exact_filter_scratch_t& x = exact_filter;
+
+    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
+        CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
+        CU(cudaStreamSynchronize(s));
+        return nullptr;
+    }
+    if (char const* e = exact_search_check(d, k)) return e; /* the refusals of search(exact = true) at this count */
+    if (char const* e = ensure_key_table(s)) return e;
+    uint32_t const sets = (uint32_t)group_count;
+    size_t const n_entries = (size_t)entries;
+
+    /* 1. the sets' live slots as sorted lists */
+    if (char const* e = listed_place_cells(*this, set_keys, n_entries, s)) return e;
+    uint64_t cells = 0;
+    CU(cudaMemcpyAsync(&cells, x.entry_at.ptr + n_entries, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (cells > 0x7FFFFFFFull) return "Too many listed rows in one call";
+    if (char const* e = listed_build_lists(*this, offsets, sets, set_keys, n_entries, cells, s)) return e;
+
+    /* 2. the queries bucketed by the count their scan needs, in query order within a bucket (the sort is stable). No count
+     * past max(k, live) is needed: that many rows hold every live entry. */
+    uint64_t const live = size - count_deleted, cap = std::max<uint64_t>(k, live);
+    int constexpr BUCKETS = 64;
+    if (char const* e = x.groups.reserve(nq)) return e;
+    if (char const* e = x.ids.reserve(nq)) return e;
+    if (char const* e = x.order.reserve(nq)) return e;
+    if (char const* e = x.sorted.reserve(nq)) return e;
+    if (char const* e = x.buckets.reserve(nq)) return e;
+    if (char const* e = x.bucket_at.reserve(BUCKETS + 1)) return e;
+    if (!groups) { /* one set: every query uses set 0 */
+        CU(cudaMemsetAsync(x.groups.ptr, 0, nq * 4, s));
+        groups = x.groups.ptr;
+    }
+    excluded_bucket_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(groups, x.list_at.ptr, (uint32_t)nq, k, cap, x.buckets.ptr);
+    CU(cudaGetLastError());
+    iota_u32_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(x.ids.ptr, nq);
+    CU(cudaGetLastError());
+    size_t temp_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, x.buckets.ptr, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, 6, s));
+    if (char const* e = x.temp.reserve(std::max<size_t>(temp_bytes, 1))) return e;
+    CU(cub::DeviceRadixSort::SortPairs(x.temp.ptr, temp_bytes, x.buckets.ptr, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, 6, s));
+    round_bounds_kernel<<<1, 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, 1, BUCKETS, x.bucket_at.ptr);
+    CU(cudaGetLastError());
+    kernel_launches += 4;
+    std::vector<uint32_t> at(BUCKETS + 1);
+    CU(cudaMemcpyAsync(at.data(), x.bucket_at.ptr, (BUCKETS + 1) * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    auto count_of = [&](int b) { return std::min<uint64_t>(1ull << b, cap); };
+    uint64_t widest = 0;
+    size_t rows = 0;
+    for (int b = 0; b < BUCKETS; ++b)
+        if (at[b + 1] > at[b]) {
+            widest = count_of(b);
+            rows = std::max<size_t>(rows, (size_t)(at[b + 1] - at[b]) * widest);
+        }
+    /* count > 256 past the tiled stage is refused here, before any output is written */
+    if (char const* e = exact_search_check(d, widest)) return e;
+
+    /* 3. the batch gathered in bucket order; per bucket the unfiltered scan at its count, then the drop into caller order */
+    size_t const vs = d.vec_stride;
+    if (char const* e = x.queries.reserve(nq * vs)) return e;
+    if (char const* e = x.keys.reserve(rows)) return e;
+    if (char const* e = x.dists.reserve(rows)) return e;
+    if (char const* e = x.counts.reserve(nq)) return e;
+    listed_gather_queries_kernel<<<(unsigned)std::min<size_t>(nq, 65535), 128, 0, s>>>(static_cast<uint8_t const*>(d_queries), stride,
+                                                                                       x.order.ptr, (uint32_t)nq, (uint32_t)d.bytes_per_vector,
+                                                                                       (uint32_t)vs, x.queries.ptr);
+    CU(cudaGetLastError());
+    kernel_launches += 1;
+    CU(cudaEventRecord(ev_begin, s));
+    for (int b = 0; b < BUCKETS; ++b) {
+        uint32_t const q0 = at[b], n_b = at[b + 1] - at[b];
+        if (!n_b) continue;
+        uint64_t const width = count_of(b);
+        if (char const* e = exact_search_device(d, stream.sm_count, x.queries.ptr + (size_t)q0 * vs, n_b, vs, width, false, true, x.keys.ptr,
+                                                x.dists.ptr, x.counts.ptr, x.exact, s))
+            return e;
+        excluded_drop_kernel<<<(n_b + 7) / 8, 256, 0, s>>>(x.order.ptr + q0, groups, x.list_at.ptr, x.rows.ptr, n_b, (uint32_t)width,
+                                                           (uint32_t)k, x.keys.ptr, x.dists.ptr, x.counts.ptr, d.keys, (uint32_t)live, d_keys,
+                                                           d_dists, d_counts, d_computed, d_visited);
+        CU(cudaGetLastError());
+        kernel_launches += 3;
+    }
+    CU(cudaEventRecord(ev_end, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end));
+    return nullptr;
+}
+
+/* host queries of any kind, host sets and host outputs, as grouped_exact_search_host serves them */
+char const* frozen_index_t::grouped_excluded_exact_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                               uint32_t const* groups, uint64_t const* offsets, size_t group_count,
+                                                               uint64_t const* set_keys, host_results_t const& out, size_t* total) {
+    std::lock_guard<std::mutex> lock(mutex);
+    if (shards) return ERR_SHARDED;
+    if (nq == 0 || k == 0) return nullptr;
+    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, EXACT_SETS)) return e;
+    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
+    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
+                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
+        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
+        return grouped_excluded_exact_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count,
+                                                    key_stage.ptr, r.keys, r.dists, r.counts, r.computed, nullptr, stream);
     });
 }
 

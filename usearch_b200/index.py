@@ -63,6 +63,8 @@ EXPORTED_SYMBOLS = [
     "usearch_b200_filtered_search_many_device", "usearch_b200_grouped_filtered_search_many",
     "usearch_b200_grouped_filtered_search_many_device", "usearch_b200_grouped_filtered_exact_search_many",
     "usearch_b200_grouped_filtered_exact_search_many_device", "usearch_b200_exact_search_device",
+    "usearch_b200_grouped_excluded_search_many", "usearch_b200_grouped_excluded_search_many_device",
+    "usearch_b200_grouped_excluded_exact_search_many", "usearch_b200_grouped_excluded_exact_search_many_device",
 ]
 
 # the fields of usearch_b200_launch_plan, in order
@@ -137,6 +139,14 @@ def load_library() -> C.CDLL:
                                                                            C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
                                                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                                            C.c_void_p, C.c_void_p, err]
+    # the excluded entries take the grouped filtered entries' arguments
+    lib.usearch_b200_grouped_excluded_search_many.restype = C.c_size_t
+    lib.usearch_b200_grouped_excluded_search_many.argtypes = lib.usearch_b200_grouped_filtered_search_many.argtypes
+    lib.usearch_b200_grouped_excluded_search_many_device.argtypes = lib.usearch_b200_grouped_filtered_search_many_device.argtypes
+    lib.usearch_b200_grouped_excluded_exact_search_many.restype = C.c_size_t
+    lib.usearch_b200_grouped_excluded_exact_search_many.argtypes = lib.usearch_b200_grouped_filtered_exact_search_many.argtypes
+    lib.usearch_b200_grouped_excluded_exact_search_many_device.argtypes = \
+        lib.usearch_b200_grouped_filtered_exact_search_many_device.argtypes
     lib.usearch_b200_tune.restype = C.c_int
     lib.usearch_b200_tune.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
     lib.usearch_b200_launch_plan.restype = C.c_int
@@ -772,13 +782,42 @@ class Index:
         ``filtered_search(vectors[i], count, key_sets[groups[i]], exact=exact)``, counters included (`last_computed` /
         `last_visited`). `key_sets` is a sequence of key iterables or arrays; ``groups=None`` gives query i the set i.
         `exact=True` scans exactly the live entries of each query's set."""
+        vectors, offsets, flat, groups, nq = self._pack_key_sets(vectors, key_sets, groups)
+        if exact:
+            return self._exact_sets(vectors, count, offsets, flat, groups, nq)
+        return self._graph_sets(vectors, count, offsets, flat, groups, nq)
+
+    def excluded_search(self, vectors: np.ndarray, count: int, excluded_keys, *, exact: bool = False) -> Union[Matches, BatchMatches]:
+        """`filtered_search` (index_dense.hpp:774-779) for the predicate "key not in excluded_keys": every live entry but
+        those stored under the given keys. `exact=True` scans exactly those entries (search_exact_ with the predicate)."""
+        if np.ndim(excluded_keys) != 1:  # a scalar is a key, not a set; a nested list is several sets
+            raise ValueError("excluded_keys must be a flat sequence of keys")
+        excluded = np.ascontiguousarray(excluded_keys, dtype=np.uint64)
         vectors = np.asarray(vectors)
-        single = vectors.ndim == 1
-        if single:
-            vectors = vectors[None, :]
-        if vectors.ndim != 2:
+        nq = vectors.shape[0] if vectors.ndim == 2 else 1
+        offsets = np.array([0, excluded.size], dtype=np.uint64)
+        if exact:
+            return self._exact_sets(vectors, count, offsets, excluded, None, nq, excluded=True)
+        return self._graph_sets(vectors, count, offsets, excluded, None, nq, excluded=True)
+
+    def grouped_excluded_search(self, vectors: np.ndarray, count: int, key_sets, groups=None, *,
+                                exact: bool = False) -> Union[Matches, BatchMatches]:
+        """`excluded_search` with a key set per query, as one call: row i equals
+        ``excluded_search(vectors[i], count, key_sets[groups[i]], exact=exact)``, counters included (`last_computed` /
+        `last_visited`). `key_sets` and `groups` as in `grouped_filtered_search`."""
+        vectors, offsets, flat, groups, nq = self._pack_key_sets(vectors, key_sets, groups)
+        if exact:
+            return self._exact_sets(vectors, count, offsets, flat, groups, nq, excluded=True)
+        return self._graph_sets(vectors, count, offsets, flat, groups, nq, excluded=True)
+
+    @staticmethod
+    def _pack_key_sets(vectors, key_sets, groups):
+        """The CSR form of a batch's key sets: (vectors, offsets u64 [G + 1], flat keys u64, groups u32 [nq], nq), checked
+        before any library call. ``groups=None`` gives query i the set i."""
+        vectors = np.asarray(vectors)
+        if vectors.ndim not in (1, 2):
             raise ValueError("Expects a matrix or a vector")
-        nq = vectors.shape[0]
+        nq = vectors.shape[0] if vectors.ndim == 2 else 1
         sets = []
         for keys in key_sets:
             if np.isscalar(keys):
@@ -799,8 +838,17 @@ class Index:
         offsets = np.zeros(len(sets) + 1, dtype=np.uint64)
         offsets[1:] = np.cumsum([len(keys) for keys in sets]) if sets else []
         flat = np.concatenate(sets) if sets else np.zeros(0, dtype=np.uint64)
-        if exact:
-            return self._exact_sets(vectors[0] if single else vectors, count, offsets, flat, groups, nq)
+        return vectors, offsets, flat, groups, nq
+
+    def _graph_sets(self, vectors: np.ndarray, count: int, offsets: np.ndarray, flat: np.ndarray, groups, nq: int, *,
+                    excluded: bool = False):
+        """usearch_b200_grouped_filtered_search_many (or its excluded twin) over CSR sets; ``groups=None`` with one set
+        means set 0 for all (excluded sets only)."""
+        single = vectors.ndim == 1
+        if single:
+            vectors = vectors[None, :]
+        if vectors.ndim != 2:
+            raise ValueError("Expects a matrix or a vector")
         if not vectors.flags.c_contiguous and vectors.strides[1] != vectors.itemsize:
             vectors = np.ascontiguousarray(vectors)
         kind = self._kind_of(vectors)
@@ -810,11 +858,13 @@ class Index:
         computed = np.zeros(nq, dtype=np.uint64)
         visited = np.zeros(nq, dtype=np.uint64)
         err = C.c_char_p()
-        self._lib.usearch_b200_grouped_filtered_search_many(
-            self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count,
-            groups.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), len(sets), flat.ctypes.data_as(C.c_void_p),
-            keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
-            computed.ctypes.data_as(C.c_void_p), visited.ctypes.data_as(C.c_void_p), C.byref(err))
+        entry = (self._lib.usearch_b200_grouped_excluded_search_many if excluded
+                 else self._lib.usearch_b200_grouped_filtered_search_many)
+        entry(self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count,
+              None if groups is None else groups.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), offsets.size - 1,
+              flat.ctypes.data_as(C.c_void_p), keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p),
+              counts.ctypes.data_as(C.c_void_p), computed.ctypes.data_as(C.c_void_p), visited.ctypes.data_as(C.c_void_p),
+              C.byref(err))
         _raise(err)
         self.last_computed, self.last_visited = computed, visited
         vm, cd = int(visited.sum()), int(computed.sum())
@@ -823,8 +873,10 @@ class Index:
             return Matches(keys[0, :n], distances[0, :n], vm, cd)
         return BatchMatches(keys, distances, counts, vm, cd)
 
-    def _exact_sets(self, vectors: np.ndarray, count: int, offsets: np.ndarray, flat: np.ndarray, groups, nq: int):
-        """usearch_b200_grouped_filtered_exact_search_many over CSR sets; ``groups=None`` with one set means set 0 for all."""
+    def _exact_sets(self, vectors: np.ndarray, count: int, offsets: np.ndarray, flat: np.ndarray, groups, nq: int, *,
+                    excluded: bool = False):
+        """usearch_b200_grouped_filtered_exact_search_many (or its excluded twin) over CSR sets; ``groups=None`` with one
+        set means set 0 for all."""
         single = vectors.ndim == 1
         if single:
             vectors = vectors[None, :]
@@ -838,11 +890,12 @@ class Index:
         counts = np.zeros(nq, dtype=np.uint64)
         computed = np.zeros(nq, dtype=np.uint64)
         err = C.c_char_p()
-        self._lib.usearch_b200_grouped_filtered_exact_search_many(
-            self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count,
-            None if groups is None else groups.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), offsets.size - 1,
-            flat.ctypes.data_as(C.c_void_p), keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p),
-            counts.ctypes.data_as(C.c_void_p), computed.ctypes.data_as(C.c_void_p), C.byref(err))
+        entry = (self._lib.usearch_b200_grouped_excluded_exact_search_many if excluded
+                 else self._lib.usearch_b200_grouped_filtered_exact_search_many)
+        entry(self._h, vectors.ctypes.data_as(C.c_void_p), nq, vectors.strides[0], SCALAR_KIND[kind], count,
+              None if groups is None else groups.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), offsets.size - 1,
+              flat.ctypes.data_as(C.c_void_p), keys.ctypes.data_as(C.c_void_p), distances.ctypes.data_as(C.c_void_p),
+              counts.ctypes.data_as(C.c_void_p), computed.ctypes.data_as(C.c_void_p), C.byref(err))
         _raise(err)
         self.last_computed, self.last_visited = computed, np.zeros(nq, dtype=np.uint64)
         cd = int(computed.sum())
@@ -1097,6 +1150,26 @@ class Index:
             _raise(err)
             return
         self._lib.usearch_b200_grouped_filtered_search_many_device(self._h, queries_ptr, nq, stride, count, groups_ptr or None,
+                                                                   offsets_ptr or None, sets_count, set_keys_ptr or None, keys_ptr,
+                                                                   distances_ptr, counts_ptr, computed_ptr or None,
+                                                                   visited_ptr or None, stream or None, C.byref(err))
+        _raise(err)
+
+    def grouped_excluded_search_device(self, queries_ptr: int, nq: int, stride: int, count: int, groups_ptr: int, offsets_ptr: int,
+                                       sets_count: int, set_keys_ptr: int, keys_ptr: int, distances_ptr: int, counts_ptr: int,
+                                       computed_ptr: int = 0, visited_ptr: int = 0, stream: int = 0, *, exact: bool = False) -> None:
+        """`grouped_excluded_search` on DEVICE memory, laid out as in `grouped_filtered_search_device`. `groups_ptr` may be
+        0 when `sets_count` is 1; with `exact=True` there is no `visited_ptr`."""
+        err = C.c_char_p()
+        if exact:
+            if visited_ptr:
+                raise ValueError("exact search has no visited_members counter")
+            self._lib.usearch_b200_grouped_excluded_exact_search_many_device(
+                self._h, queries_ptr, nq, stride, count, groups_ptr or None, offsets_ptr or None, sets_count, set_keys_ptr or None,
+                keys_ptr, distances_ptr, counts_ptr, computed_ptr or None, stream or None, C.byref(err))
+            _raise(err)
+            return
+        self._lib.usearch_b200_grouped_excluded_search_many_device(self._h, queries_ptr, nq, stride, count, groups_ptr or None,
                                                                    offsets_ptr or None, sets_count, set_keys_ptr or None, keys_ptr,
                                                                    distances_ptr, counts_ptr, computed_ptr or None,
                                                                    visited_ptr or None, stream or None, C.byref(err))
