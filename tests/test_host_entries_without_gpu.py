@@ -1,6 +1,7 @@
 """The C search entries on host buffers, called through ctypes past the Python checks, on an index without members: each
 answers with padded empty rows and returns a total of 0, with or without `counts`, and the grouped entries refuse
-malformed key sets with their own messages, in their own order, before writing any output. None of this needs a device."""
+malformed key sets with their own messages, in their own order, before writing any output: the allowed and excluded sets,
+graph and exact, through the one host body they share. None of this needs a device."""
 import ctypes as C
 
 import numpy as np
@@ -30,12 +31,15 @@ def lib():
     lib.usearch_init.restype = p
     lib.usearch_free.argtypes = [p, err]
     for name in ("usearch_b200_filtered_search_many", "usearch_filtered_search", "usearch_b200_grouped_filtered_search_many",
-                 "usearch_b200_grouped_filtered_exact_search_many", "usearch_b200_exact_search_many"):
+                 "usearch_b200_grouped_filtered_exact_search_many", "usearch_b200_grouped_excluded_search_many",
+                 "usearch_b200_grouped_excluded_exact_search_many", "usearch_b200_exact_search_many"):
         getattr(lib, name).restype = n
     lib.usearch_b200_filtered_search_many.argtypes = [p, p, n, n, C.c_int, n, p, n, p, p, p, p, p, err]
     lib.usearch_filtered_search.argtypes = [p, p, C.c_int, n, FILTER, p, p, p, err]
     lib.usearch_b200_grouped_filtered_search_many.argtypes = [p, p, n, n, C.c_int, n, p, p, n, p, p, p, p, p, p, err]
     lib.usearch_b200_grouped_filtered_exact_search_many.argtypes = [p, p, n, n, C.c_int, n, p, p, n, p, p, p, p, p, err]
+    lib.usearch_b200_grouped_excluded_search_many.argtypes = lib.usearch_b200_grouped_filtered_search_many.argtypes
+    lib.usearch_b200_grouped_excluded_exact_search_many.argtypes = lib.usearch_b200_grouped_filtered_exact_search_many.argtypes
     lib.usearch_b200_exact_search_many.argtypes = [p, p, n, n, C.c_int, n, p, p, p, err]
     return lib
 
@@ -56,14 +60,15 @@ F32 = 1  # usearch_scalar_f32_k
 KEEP_ALL = FILTER(lambda key, state: 1)
 
 
-def _grouped(lib, index, exact, groups, offsets, set_keys):
-    """the grouped entry, as call(keys, dists, counts, computed, visited, error)"""
+def _grouped(lib, index, excluded, exact, groups, offsets, set_keys):
+    """the grouped entry of the mode, as call(keys, dists, counts, computed, visited, error)"""
     def call(keys, dists, counts, computed, visited, error):
         head = (index, QUERIES.ctypes.data, NQ, DIM * 4, F32, K, _ptr(groups), _ptr(offsets), len(offsets) - 1, _ptr(set_keys),
                 _ptr(keys), _ptr(dists), _ptr(counts), _ptr(computed))
+        form = "excluded" if excluded else "filtered"
         if exact:
-            return lib.usearch_b200_grouped_filtered_exact_search_many(*head, error)
-        return lib.usearch_b200_grouped_filtered_search_many(*head, _ptr(visited), error)
+            return getattr(lib, f"usearch_b200_grouped_{form}_exact_search_many")(*head, error)
+        return getattr(lib, f"usearch_b200_grouped_{form}_search_many")(*head, _ptr(visited), error)
     return call
 
 
@@ -79,16 +84,20 @@ def _entry(lib, index, name):
         return 1, (), lambda k, d, c, cm, v, e: lib.usearch_filtered_search(index, QUERIES.ctypes.data, F32, K, KEEP_ALL, None,
                                                                             _ptr(k), _ptr(d), e)
     if name == "grouped_filtered_search_many":
-        return NQ, ("computed", "visited"), _grouped(lib, index, False, *sets)
+        return NQ, ("computed", "visited"), _grouped(lib, index, False, False, *sets)
     if name == "grouped_filtered_exact_search_many":
-        return NQ, ("computed",), _grouped(lib, index, True, *sets)
+        return NQ, ("computed",), _grouped(lib, index, False, True, *sets)
+    if name == "grouped_excluded_search_many":
+        return NQ, ("computed", "visited"), _grouped(lib, index, True, False, *sets)
+    if name == "grouped_excluded_exact_search_many":
+        return NQ, ("computed",), _grouped(lib, index, True, True, *sets)
     assert name == "exact_search_many"
     return NQ, (), lambda k, d, c, cm, v, e: lib.usearch_b200_exact_search_many(index, QUERIES.ctypes.data, NQ, DIM * 4, F32, K,
                                                                                 _ptr(k), _ptr(d), _ptr(c), e)
 
 
 ENTRIES = ["filtered_search_many", "filtered_search", "grouped_filtered_search_many", "grouped_filtered_exact_search_many",
-           "exact_search_many"]
+           "exact_search_many", "grouped_excluded_search_many", "grouped_excluded_exact_search_many"]
 
 
 @pytest.mark.parametrize("with_counts", [True, False])
@@ -108,7 +117,9 @@ def test_an_index_without_members_answers_padded_rows_and_a_zero_total(lib, inde
     assert (visited == 0).all() == ("visited" in counters)
 
 
-@pytest.mark.parametrize("exact", [False, True])
+# the allowed forms keep the ids "False" / "True" (exact) they had before the excluded forms joined
+@pytest.mark.parametrize("excluded,exact", [(False, False), (False, True), (True, False), (True, True)],
+                         ids=["False", "True", "excluded-False", "excluded-True"])
 @pytest.mark.parametrize("groups,offsets,message", [
     ([0, 1, 0], [1, 2, 3], BAD_OFFSETS),    # offsets not starting at 0
     ([0, 1, 0], [0, 2, 1], BAD_OFFSETS),    # offsets decreasing
@@ -119,9 +130,9 @@ def test_an_index_without_members_answers_padded_rows_and_a_zero_total(lib, inde
     ([0, 0, 0], [0], NO_SETS),              # zero sets
     (None, [0], NO_SETS),                   # ... checked first
 ])
-def test_grouped_entries_refuse_malformed_sets_before_writing(lib, index, exact, groups, offsets, message):
+def test_grouped_entries_refuse_malformed_sets_before_writing(lib, index, excluded, exact, groups, offsets, message):
     groups = None if groups is None else np.array(groups, np.uint32)
-    call = _grouped(lib, index, exact, groups, np.array(offsets, np.uint64), np.array([1, 2, 3], np.uint64))
+    call = _grouped(lib, index, excluded, exact, groups, np.array(offsets, np.uint64), np.array([1, 2, 3], np.uint64))
     keys, dists = np.full((NQ, K), 7, np.uint64), np.zeros((NQ, K), np.float32)
     counts, computed, visited = np.full(NQ, 9, np.uintp), np.full(NQ, 9, np.uint64), np.full(NQ, 9, np.uint64)
     err = C.c_char_p()

@@ -197,11 +197,10 @@ usearch_index_t usearch_init(usearch_init_options_t* options, usearch_error_t* e
 
 void usearch_free(usearch_index_t index, usearch_error_t*) { delete as_index(index); }
 
-size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table, the grouped filter's bitmap
-                                                                        rows and the exact filter's scratch count once they exist */
+size_t usearch_memory_usage(usearch_index_t index, usearch_error_t*) { /* the device key table and the key-set searches'
+                                                                        scratch count once they exist */
     frozen_index_t const* ix = as_index(index);
-    return ix->hbm_bytes + ix->key_table.cells.capacity * sizeof(key_cell_t) + ix->group_bits.capacity * sizeof(uint32_t) +
-           ix->exact_filter.bytes();
+    return ix->hbm_bytes + ix->key_table.cells.capacity * sizeof(key_cell_t) + ix->key_set_scratch.bytes();
 }
 
 char const* usearch_hardware_acceleration(usearch_index_t, usearch_error_t*) { return "sm_90a"; }
@@ -393,11 +392,11 @@ size_t usearch_b200_grouped_filtered_search_many(usearch_index_t index, void con
                                                  size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
                                                  usearch_error_t* error) {
     return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
-        return as_index(index)->grouped_filtered_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count,
-                                                             set_keys,
-                                                             host_results_t{keys, count * 8, distances, count * 4, counts,
-                                                                            computed_distances, visited_members},
-                                                             total);
+        return as_index(index)->key_set_search_host(queries, queries_count, queries_stride, qs, count,
+                                                    key_sets_t{groups, offsets, sets_count, set_keys}, false, false,
+                                                    host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances,
+                                                                   visited_members},
+                                                    total);
     });
 }
 
@@ -408,8 +407,8 @@ void usearch_b200_grouped_filtered_search_many_device(usearch_index_t index, voi
                                                       uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                                       usearch_error_t* error) {
     device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
-        return ix->grouped_filtered_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
-                                                  keys, distances, counts, computed_distances, visited_members, s);
+        return ix->key_set_search_device(queries, queries_count, queries_stride, count, key_sets_t{groups, offsets, sets_count, set_keys},
+                                         false, false, device_results_t{keys, distances, counts, computed_distances, visited_members}, s);
     });
 }
 
@@ -420,10 +419,9 @@ size_t usearch_b200_grouped_filtered_exact_search_many(usearch_index_t index, vo
                                                        usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
                                                        size_t* counts, uint64_t* computed_distances, usearch_error_t* error) {
     return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
-        return as_index(index)->grouped_exact_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count,
-                                                          set_keys,
-                                                          host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances},
-                                                          total);
+        return as_index(index)->key_set_search_host(queries, queries_count, queries_stride, qs, count,
+                                                    key_sets_t{groups, offsets, sets_count, set_keys}, false, true,
+                                                    host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances}, total);
     });
 }
 
@@ -433,8 +431,8 @@ void usearch_b200_grouped_filtered_exact_search_many_device(usearch_index_t inde
                                                             usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                                             uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error) {
     device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
-        return ix->grouped_exact_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys, keys,
-                                               distances, counts, computed_distances, nullptr, s);
+        return ix->key_set_search_device(queries, queries_count, queries_stride, count, key_sets_t{groups, offsets, sets_count, set_keys},
+                                         false, true, device_results_t{keys, distances, counts, computed_distances, nullptr}, s);
     });
 }
 
@@ -446,11 +444,11 @@ size_t usearch_b200_grouped_excluded_search_many(usearch_index_t index, void con
                                                  size_t* counts, uint64_t* computed_distances, uint64_t* visited_members,
                                                  usearch_error_t* error) {
     return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
-        return as_index(index)->grouped_excluded_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets, sets_count,
-                                                             set_keys,
-                                                             host_results_t{keys, count * 8, distances, count * 4, counts,
-                                                                            computed_distances, visited_members},
-                                                             total);
+        return as_index(index)->key_set_search_host(queries, queries_count, queries_stride, qs, count,
+                                                    key_sets_t{groups, offsets, sets_count, set_keys}, true, false,
+                                                    host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances,
+                                                                   visited_members},
+                                                    total);
     });
 }
 
@@ -461,8 +459,8 @@ void usearch_b200_grouped_excluded_search_many_device(usearch_index_t index, voi
                                                       uint32_t* computed_distances, uint32_t* visited_members, void* cuda_stream,
                                                       usearch_error_t* error) {
     device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
-        return ix->grouped_excluded_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
-                                                  keys, distances, counts, computed_distances, visited_members, s);
+        return ix->key_set_search_device(queries, queries_count, queries_stride, count, key_sets_t{groups, offsets, sets_count, set_keys},
+                                         true, false, device_results_t{keys, distances, counts, computed_distances, visited_members}, s);
     });
 }
 
@@ -472,11 +470,9 @@ size_t usearch_b200_grouped_excluded_exact_search_many(usearch_index_t index, vo
                                                        usearch_key_t const* set_keys, usearch_key_t* keys, usearch_distance_t* distances,
                                                        size_t* counts, uint64_t* computed_distances, usearch_error_t* error) {
     return host_search(query_kind, error, [&](uint32_t qs, size_t* total) {
-        return as_index(index)->grouped_excluded_exact_search_host(queries, queries_count, queries_stride, qs, count, groups, offsets,
-                                                                   sets_count, set_keys,
-                                                                   host_results_t{keys, count * 8, distances, count * 4, counts,
-                                                                                  computed_distances},
-                                                                   total);
+        return as_index(index)->key_set_search_host(queries, queries_count, queries_stride, qs, count,
+                                                    key_sets_t{groups, offsets, sets_count, set_keys}, true, true,
+                                                    host_results_t{keys, count * 8, distances, count * 4, counts, computed_distances}, total);
     });
 }
 
@@ -486,8 +482,8 @@ void usearch_b200_grouped_excluded_exact_search_many_device(usearch_index_t inde
                                                             usearch_key_t* keys, usearch_distance_t* distances, uint32_t* counts,
                                                             uint32_t* computed_distances, void* cuda_stream, usearch_error_t* error) {
     device_search(index, cuda_stream, error, [&](frozen_index_t* ix, cudaStream_t s) {
-        return ix->grouped_excluded_exact_search_device(queries, queries_count, queries_stride, count, groups, offsets, sets_count, set_keys,
-                                                        keys, distances, counts, computed_distances, nullptr, s);
+        return ix->key_set_search_device(queries, queries_count, queries_stride, count, key_sets_t{groups, offsets, sets_count, set_keys},
+                                         true, true, device_results_t{keys, distances, counts, computed_distances, nullptr}, s);
     });
 }
 

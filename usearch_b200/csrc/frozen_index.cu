@@ -66,8 +66,7 @@ void frozen_index_t::release_device() {
     host_keys.clear();
     key_map.clear();
     key_table = key_table_t{};
-    group_bits = device_buffer_t<uint32_t>{};
-    exact_filter = exact_filter_scratch_t{};
+    key_set_scratch = key_set_scratch_t{};
     keys_generation += 1;
 }
 

@@ -106,6 +106,14 @@ struct device_results_t {
     uint32_t* computed;
     uint32_t* visited;
 };
+/* the key sets of a key-set search, as CSR: set g holds keys[offsets[g] .. offsets[g + 1]), query i uses set groups[i].
+ * `groups` may be NULL with one set (every query uses set 0) except in the allowed graph form. */
+struct key_sets_t {
+    uint32_t const* groups;
+    uint64_t const* offsets; /* count + 1 */
+    size_t count;
+    uint64_t const* keys;
+};
 /* the device call of a host search: queries in the index's kind, rows `stride` bytes apart, outputs in `out` */
 using device_search_t = std::function<char const*(void const* d_queries, size_t stride, device_results_t const& out)>;
 /* index_gt::search on an empty index: no matches, no error (index.hpp:3036-3037); every row key 0 and a signalling NaN */
@@ -261,62 +269,27 @@ struct frozen_index_t {
     char const* filtered_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, uint64_t const* allowed,
                                      size_t allowed_count, host_results_t const& out, size_t* total);
 
-    /* grouped_filter.cu: a batch whose query i is filtered by key set groups[i], the sets given as CSR (offsets[G + 1] into
-     * set_keys), every pointer in device memory. One bitmap row per set, built from the key table; rows of as many sets
-     * as `group_bitmap_mb` allows per launch. */
-    device_buffer_t<uint32_t> group_bits; /* the rows of one round; counted by memory_usage */
-    device_buffer_t<uint32_t> group_order, group_sorted, group_ids, group_bounds, group_flag;
-    device_buffer_t<uint8_t> group_sort_temp;
-    device_buffer_t<uint64_t> group_offsets; /* a host entry's upload of `offsets` (its keys go to `key_stage`) */
-    device_buffer_t<uint32_t> group_upload;   /* ... and of `groups` */
-    char const* grouped_filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                               uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
-                                               float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                               cudaStream_t s);
-    char const* grouped_filtered_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                             uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                             host_results_t const& out, size_t* total);
-    /* excluded sets: query i searches the live entries whose key is NOT in set groups[i]; each row is the complement bitmap,
-     * all ones less the set's slots. `groups` may be NULL when group_count == 1. */
-    char const* grouped_excluded_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                               uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
-                                               float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                               cudaStream_t s);
-    char const* grouped_excluded_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                             uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                             host_results_t const& out, size_t* total);
-    /* both graph forms: rows that allow the sets' slots, or (`excluded`) rows that allow every slot but them */
-    char const* grouped_rows_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                           uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, bool excluded,
-                                           uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                           cudaStream_t s);
-
-    /* grouped_filter.cu, exact form: search_exact_ over the live slots of each query's set (LISTED exact kernels). `groups`
-     * may be NULL when group_count == 1. The scratch is counted by memory_usage and freed by clear. */
-    struct exact_filter_scratch_t {
-        device_buffer_t<uint32_t> rows, list_at, query_at, per_set, item_at, order, sorted, ids, groups, scalars, counts;
-        device_buffer_t<uint32_t> buckets, bucket_at; /* the exact excluded search's buckets: per query, and their bounds */
+    /* grouped_filter.cu: key-set searches, each query under its own set of a CSR list (key_sets_t). Query i searches the
+     * live entries whose key is in set groups[i], or (`excluded`) whose key is not, through the graph or (`exact`) by brute
+     * force: one bitmap row per set from the key table for the graph, one slot list per set for the exact forms. */
+    struct key_set_scratch_t {
+        device_buffer_t<uint32_t> bits;           /* graph: the rows of one round, as many as `group_bitmap_mb` allows */
+        device_buffer_t<uint32_t> flag, groups;   /* the device checks' flag; `groups` of a host entry, or zeros for one set */
+        device_buffer_t<uint64_t> offsets;        /* a host entry's `offsets` (its keys go to `key_stage`) */
+        device_buffer_t<uint32_t> ids, order, sorted, bounds; /* query ids sorted by set or bucket, and the bounds of the runs */
+        device_buffer_t<uint8_t> temp;            /* cub's */
+        device_buffer_t<uint32_t> rows, list_at, query_at, per_set, item_at, scalars, counts, buckets; /* exact: slot lists, items */
         device_buffer_t<uint64_t> entry_counts, entry_at, words, words_sorted, keys;
         device_buffer_t<exact_item_t> items;
-        device_buffer_t<uint8_t> temp, queries, exact;
+        device_buffer_t<uint8_t> queries, exact;
         device_buffer_t<float> dists;
         size_t bytes() const;
-    } exact_filter;
-    char const* grouped_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                            uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
-                                            float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited, cudaStream_t s);
-    char const* grouped_exact_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                          uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                          host_results_t const& out, size_t* total);
-    /* exact excluded search: search_exact_ over the live slots outside each query's set, as the unfiltered scan's top-(k + e)
-     * less the set's e live slots. Same scratch as the exact filtered form. */
-    char const* grouped_excluded_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                                     uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
-                                                     float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                                     cudaStream_t s);
-    char const* grouped_excluded_exact_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                                   uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                   uint64_t const* set_keys, host_results_t const& out, size_t* total);
+    } key_set_scratch; /* all of it counted by memory_usage and freed by clear */
+    char const* key_set_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, key_sets_t const& sets, bool excluded,
+                                      bool exact, device_results_t const& out, cudaStream_t s);
+    /* the same from host queries of any kind, host sets and host outputs */
+    char const* key_set_search_host(void const* queries, size_t nq, size_t stride, uint32_t query_scalar, size_t k, key_sets_t const& sets,
+                                    bool excluded, bool exact, host_results_t const& out, size_t* total);
 
     /* searches */
     /* grouped: plan for the GROUPED kernel (its occupancy) */

@@ -16,6 +16,9 @@
  *  Excluded sets (query i searches every live entry whose key is NOT in its set) reuse both: on the graph each row starts
  *  all ones and loses the set's slots; the exact form runs the unfiltered scan at count k + e (e = the live slots of the
  *  set, from its slot list) and drops the set's slots from each row.
+ *
+ *  All four modes enter through key_set_search_host / key_set_search_device, which share the checks, the empty-index
+ *  answer and the key table, and keep their scratch in frozen_index_t::key_set_scratch.
  */
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -42,6 +45,28 @@ enum : uint32_t { BAD_GROUP = 1, BAD_OFFSETS = 2 };
 
 unsigned grid_for(size_t items, int sm_count) { return (unsigned)std::max<size_t>(1, std::min<size_t>((items + 255) / 256, (size_t)sm_count * 16)); }
 
+/* the bits a radix sort needs for values below `values` (at least 1) */
+int bits_for(size_t values) {
+    int bits = 1;
+    while (bits < 32 && (values - 1) >> bits) ++bits;
+    return bits;
+}
+
+/* the first i of [lo, hi) with !less(i), for a `less` that holds on a prefix of the range (hi when it holds on all) */
+template <typename Less> __device__ __forceinline__ uint32_t lower_bound(uint32_t lo, uint32_t hi, Less less) {
+    while (lo < hi) {
+        uint32_t const mid = (lo + hi) >> 1;
+        if (less(mid)) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+/* the set g of [g0, g1) holding CSR entry e: offsets[g] <= e < offsets[g + 1], for offsets[g0] <= e < offsets[g1] */
+__device__ __forceinline__ uint32_t set_of_entry(uint64_t const* offsets, uint32_t g0, uint32_t g1, uint64_t e) {
+    return lower_bound(g0 + 1, g1, [&](uint32_t g) { return offsets[g] <= e; }) - 1;
+}
+
 __global__ void grouped_validate_kernel(uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count, uint32_t* flag) {
     size_t const n = max(nq, group_count);
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -51,45 +76,47 @@ __global__ void grouped_validate_kernel(uint32_t const* groups, size_t nq, uint6
     }
 }
 
-/* what each grouped entry accepts beyond the CSR rules both share */
+/* what each mode accepts beyond the CSR rules all share */
 struct key_set_rules_t {
     uint64_t max_sets;    /* refused from this many sets on */
     bool groups_optional; /* `groups` may be NULL when there is one set: every query uses set 0 */
     uint64_t max_entries; /* keys in all the sets */
 };
 constexpr key_set_rules_t GRAPH_SETS{0xFFFFFFFFull, false, UINT64_MAX};
-constexpr key_set_rules_t EXACT_SETS{0x7FFFFFFFull, true, 0x7FFFFFFFull};
 constexpr key_set_rules_t EXCLUDED_GRAPH_SETS{0xFFFFFFFFull, true, UINT64_MAX};
+constexpr key_set_rules_t EXACT_SETS{0x7FFFFFFFull, true, 0x7FFFFFFFull}; /* both exact forms */
+key_set_rules_t const& rules_of(bool excluded, bool exact) { return exact ? EXACT_SETS : excluded ? EXCLUDED_GRAPH_SETS : GRAPH_SETS; }
 
 /* the sets of a host entry, checked before anything is uploaded (the offsets size the upload) */
-char const* check_key_sets_host(uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count, key_set_rules_t const& rules) {
-    if (group_count == 0) return ERR_NO_SETS;
-    if (!groups && !(rules.groups_optional && group_count == 1)) return ERR_NO_GROUPS;
-    if (offsets[0] != 0) return ERR_OFFSETS;
-    for (size_t g = 0; g < group_count; ++g)
-        if (offsets[g + 1] < offsets[g]) return ERR_OFFSETS;
-    if (groups)
+char const* check_key_sets_host(key_sets_t const& sets, size_t nq, key_set_rules_t const& rules) {
+    if (sets.count == 0) return ERR_NO_SETS;
+    if (!sets.groups && !(rules.groups_optional && sets.count == 1)) return ERR_NO_GROUPS;
+    if (sets.offsets[0] != 0) return ERR_OFFSETS;
+    for (size_t g = 0; g < sets.count; ++g)
+        if (sets.offsets[g + 1] < sets.offsets[g]) return ERR_OFFSETS;
+    if (sets.groups)
         for (size_t i = 0; i < nq; ++i)
-            if (groups[i] >= group_count) return ERR_GROUP;
+            if (sets.groups[i] >= sets.count) return ERR_GROUP;
     return nullptr;
 }
 
 /* the sets of a device entry, checked on the device before any output is written: one launch, one read-back, which also
  * brings back the number of keys in all the sets */
-char const* check_key_sets_device(frozen_index_t& ix, uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count,
-                                  key_set_rules_t const& rules, uint64_t* entries, cudaStream_t s) {
-    if (group_count == 0) return ERR_NO_SETS;
-    if (group_count >= rules.max_sets) return "Too many key sets in one call";
-    if (!groups && !(rules.groups_optional && group_count == 1)) return ERR_NO_GROUPS;
-    if (char const* e = ix.group_flag.reserve(1)) return e;
-    CU(cudaMemsetAsync(ix.group_flag.ptr, 0, 4, s));
-    grouped_validate_kernel<<<grid_for(std::max(nq, group_count), ix.stream.sm_count), 256, 0, s>>>(groups, groups ? nq : 0, offsets,
-                                                                                                    group_count, ix.group_flag.ptr);
+char const* check_key_sets_device(frozen_index_t& ix, key_sets_t const& sets, size_t nq, key_set_rules_t const& rules, uint64_t* entries,
+                                  cudaStream_t s) {
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
+    if (sets.count == 0) return ERR_NO_SETS;
+    if (sets.count >= rules.max_sets) return "Too many key sets in one call";
+    if (!sets.groups && !(rules.groups_optional && sets.count == 1)) return ERR_NO_GROUPS;
+    if (char const* e = x.flag.reserve(1)) return e;
+    CU(cudaMemsetAsync(x.flag.ptr, 0, 4, s));
+    grouped_validate_kernel<<<grid_for(std::max(nq, sets.count), ix.stream.sm_count), 256, 0, s>>>(sets.groups, sets.groups ? nq : 0, sets.offsets,
+                                                                                                   sets.count, x.flag.ptr);
     CU(cudaGetLastError());
     ix.kernel_launches += 1;
     uint32_t flag = 0;
-    CU(cudaMemcpyAsync(&flag, ix.group_flag.ptr, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(entries, offsets + group_count, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&flag, x.flag.ptr, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(entries, sets.offsets + sets.count, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (flag & BAD_GROUP) return ERR_GROUP;
     if (flag & BAD_OFFSETS) return ERR_OFFSETS;
@@ -97,14 +124,14 @@ char const* check_key_sets_device(frozen_index_t& ix, uint32_t const* groups, si
     return nullptr;
 }
 
-/* a host entry's sets to the device: `groups` (when given) to group_upload, `offsets` to group_offsets, the keys to key_stage */
-char const* upload_key_sets(frozen_index_t& ix, uint32_t const* groups, size_t nq, uint64_t const* offsets, size_t group_count,
-                            uint64_t const* set_keys) {
-    if (char const* e = ix.group_upload.reserve(nq)) return e;
-    if (char const* e = ix.group_offsets.reserve(group_count + 1)) return e;
-    if (char const* e = ix.stage_keys(set_keys, offsets[group_count])) return e;
-    if (groups) CU(cudaMemcpyAsync(ix.group_upload.ptr, groups, nq * 4, cudaMemcpyHostToDevice, ix.stream));
-    CU(cudaMemcpyAsync(ix.group_offsets.ptr, offsets, (group_count + 1) * 8, cudaMemcpyHostToDevice, ix.stream));
+/* a host entry's sets to the device: `groups` (when given) to x.groups, `offsets` to x.offsets, the keys to key_stage */
+char const* upload_key_sets(frozen_index_t& ix, key_sets_t const& sets, size_t nq) {
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
+    if (char const* e = x.groups.reserve(nq)) return e;
+    if (char const* e = x.offsets.reserve(sets.count + 1)) return e;
+    if (char const* e = ix.stage_keys(sets.keys, sets.offsets[sets.count])) return e;
+    if (sets.groups) CU(cudaMemcpyAsync(x.groups.ptr, sets.groups, nq * 4, cudaMemcpyHostToDevice, ix.stream));
+    CU(cudaMemcpyAsync(x.offsets.ptr, sets.offsets, (sets.count + 1) * 8, cudaMemcpyHostToDevice, ix.stream));
     return nullptr;
 }
 
@@ -115,13 +142,7 @@ __global__ void grouped_bits_kernel(key_cell_t const* cells, uint64_t mask, uint
                                     uint32_t* rows) {
     uint64_t const begin = offsets[g0], end = offsets[g1];
     for (uint64_t e = begin + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < end; e += (uint64_t)gridDim.x * blockDim.x) {
-        uint32_t lo = g0 + 1, hi = g1; /* the first set past entry e: offsets[lo] > e */
-        while (lo < hi) {
-            uint32_t const mid = (lo + hi) >> 1;
-            if (offsets[mid] > e) hi = mid;
-            else lo = mid + 1;
-        }
-        uint32_t* const row = rows + (size_t)(lo - 1 - g0) * words;
+        uint32_t* const row = rows + (size_t)(set_of_entry(offsets, g0, g1, e) - g0) * words;
         uint64_t const key = set_keys[e];
         if (key == free_key) {
             if (deleted_bits)
@@ -142,13 +163,7 @@ __global__ void excluded_bits_kernel(key_cell_t const* cells, uint64_t mask, uin
                                      uint32_t g1, uint32_t words, uint32_t* rows) {
     uint64_t const begin = offsets[g0], end = offsets[g1];
     for (uint64_t e = begin + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < end; e += (uint64_t)gridDim.x * blockDim.x) {
-        uint32_t lo = g0 + 1, hi = g1; /* the first set past entry e: offsets[lo] > e */
-        while (lo < hi) {
-            uint32_t const mid = (lo + hi) >> 1;
-            if (offsets[mid] > e) hi = mid;
-            else lo = mid + 1;
-        }
-        uint32_t* const row = rows + (size_t)(lo - 1 - g0) * words;
+        uint32_t* const row = rows + (size_t)(set_of_entry(offsets, g0, g1, e) - g0) * words;
         key_table_for_each(cells, mask, set_keys[e], [&](uint32_t s) { atomicAnd(row + (s >> 5), ~(1u << (s & 31))); });
     }
 }
@@ -157,32 +172,30 @@ __global__ void iota_u32_kernel(uint32_t* out, size_t n) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) out[i] = (uint32_t)i;
 }
 
-/* bounds[r] = the first position of `sorted` holding a set id >= r * per_round, for r <= rounds */
+/* bounds[r] = the first position of `sorted` holding a value >= r * per_round, for r <= rounds */
 __global__ void round_bounds_kernel(uint32_t const* sorted, uint32_t nq, uint32_t per_round, uint32_t rounds, uint32_t* bounds) {
     uint32_t const r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r > rounds) return;
     uint64_t const first = (uint64_t)r * per_round;
-    uint32_t lo = 0, hi = nq;
-    while (lo < hi) {
-        uint32_t const mid = (lo + hi) >> 1;
-        if (sorted[mid] < first) lo = mid + 1;
-        else hi = mid;
-    }
-    bounds[r] = lo;
+    bounds[r] = lower_bound(0, nq, [&](uint32_t p) { return sorted[p] < first; });
+}
+
+/* x.order = the query ids 0 .. nq - 1 stably sorted by key[id] over bits [0, end_bit), x.sorted = their keys. Nothing waits. */
+char const* sort_queries(frozen_index_t& ix, uint32_t const* key, size_t nq, int end_bit, cudaStream_t s) {
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
+    if (char const* e = x.ids.reserve(nq)) return e;
+    if (char const* e = x.order.reserve(nq)) return e;
+    if (char const* e = x.sorted.reserve(nq)) return e;
+    iota_u32_kernel<<<grid_for(nq, ix.stream.sm_count), 256, 0, s>>>(x.ids.ptr, nq);
+    CU(cudaGetLastError());
+    size_t temp_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, key, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, end_bit, s));
+    if (char const* e = x.temp.reserve(std::max<size_t>(temp_bytes, 1))) return e;
+    CU(cub::DeviceRadixSort::SortPairs(x.temp.ptr, temp_bytes, key, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, end_bit, s));
+    return nullptr;
 }
 
 /* ---- exact filtered search ---- */
-
-/* the first g of [lo, hi) with offsets[g + 1] > e: the set holding CSR entry e */
-__device__ __forceinline__ uint32_t set_of_entry(uint64_t const* offsets, uint32_t sets, uint64_t e) {
-    uint32_t lo = 1, hi = sets;
-    while (lo < hi) {
-        uint32_t const mid = (lo + hi) >> 1;
-        if (offsets[mid] > e) hi = mid;
-        else lo = mid + 1;
-    }
-    return lo - 1;
-}
 
 /* counts[e] = the live slots under set_keys[e]; the table holds no slot of the free key, so removed slots never count. The
  * counts are 64-bit so that their scan sums in 64 bits (cub takes the sum's type from its input). */
@@ -198,7 +211,7 @@ __global__ void listed_count_kernel(key_cell_t const* cells, uint64_t mask, uint
 __global__ void listed_write_kernel(key_cell_t const* cells, uint64_t mask, uint64_t const* offsets, uint32_t sets, uint64_t const* set_keys,
                                     size_t entries, uint64_t const* at, uint64_t* words) {
     for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < entries; e += (size_t)gridDim.x * blockDim.x) {
-        uint64_t const set = set_of_entry(offsets, sets + 1, e);
+        uint64_t const set = set_of_entry(offsets, 0, sets, e);
         uint64_t p = at[e];
         key_table_for_each(cells, mask, set_keys[e], [&](uint32_t s) { words[p++] = set << 32 | s; });
     }
@@ -210,30 +223,15 @@ __global__ void listed_rows_kernel(uint64_t const* words, uint32_t const* unique
                                    uint32_t* list_at) {
     uint32_t const n = *unique_count;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < bound; i += gridDim.x * blockDim.x) rows[i] = i < n ? (uint32_t)words[i] : 0u;
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g <= sets; g += gridDim.x * blockDim.x) {
-        uint32_t lo = 0, hi = n;
-        while (lo < hi) {
-            uint32_t const mid = (lo + hi) >> 1;
-            if ((words[mid] >> 32) < g) lo = mid + 1;
-            else hi = mid;
-        }
-        list_at[g] = lo;
-    }
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g <= sets; g += gridDim.x * blockDim.x)
+        list_at[g] = lower_bound(0, n, [&](uint32_t i) { return (words[i] >> 32) < g; });
 }
 
 /* query_at[g] = the first position of `sorted` (set ids of the queries, ascending) holding g or more; per_set[g] = the
  * work items set g needs at `qpc` queries per item (per_set[sets] = 0, so an exclusive scan ends at the item count) */
 __global__ void listed_item_counts_kernel(uint32_t const* sorted, uint32_t nq, uint32_t sets, uint32_t qpc, uint32_t* query_at, uint32_t* per_set) {
     for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g <= sets; g += gridDim.x * blockDim.x) {
-        auto first = [&](uint32_t v) {
-            uint32_t lo = 0, hi = nq;
-            while (lo < hi) {
-                uint32_t const mid = (lo + hi) >> 1;
-                if (sorted[mid] < v) lo = mid + 1;
-                else hi = mid;
-            }
-            return lo;
-        };
+        auto first = [&](uint32_t v) { return lower_bound(0, nq, [&](uint32_t p) { return sorted[p] < v; }); };
         uint32_t const a = first(g);
         query_at[g] = a;
         per_set[g] = g < sets ? (first(g + 1) - a + qpc - 1) / qpc : 0u;
@@ -312,13 +310,8 @@ __global__ void excluded_drop_kernel(uint32_t const* order, uint32_t const* grou
         bool keep = false;
         if (j < n) {
             slot = (uint32_t)slots[(size_t)p * width + j];
-            uint32_t lo = 0, hi = e;
-            while (lo < hi) {
-                uint32_t const mid = (lo + hi) >> 1;
-                if (list[mid] < slot) lo = mid + 1;
-                else hi = mid;
-            }
-            keep = lo == e || list[lo] != slot;
+            uint32_t const at = lower_bound(0, e, [&](uint32_t m) { return list[m] < slot; });
+            keep = at == e || list[at] != slot;
         }
         uint32_t const ballot = __ballot_sync(0xFFFFFFFFu, keep);
         uint32_t const at = kept + __popc(ballot & ((1u << lane) - 1u));
@@ -340,191 +333,96 @@ __global__ void excluded_drop_kernel(uint32_t const* order, uint32_t const* grou
     }
 }
 
-} // namespace
+/* ---- the three searches, past the shared checks: `sets.groups` is never NULL and the key table is current ---- */
 
-char const* frozen_index_t::grouped_filtered_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
-                                                           uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                           uint64_t const* set_keys, uint64_t* d_keys, float* d_dists,
-                                                           uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                                           cudaStream_t s) {
-    return grouped_rows_search_device(d_queries, nq, stride, k, groups, offsets, group_count, set_keys, false, d_keys, d_dists, d_counts,
-                                      d_computed, d_visited, s);
-}
-
-char const* frozen_index_t::grouped_excluded_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
-                                                           uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                           uint64_t const* set_keys, uint64_t* d_keys, float* d_dists,
-                                                           uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                                           cudaStream_t s) {
-    return grouped_rows_search_device(d_queries, nq, stride, k, groups, offsets, group_count, set_keys, true, d_keys, d_dists, d_counts,
-                                      d_computed, d_visited, s);
-}
-
-char const* frozen_index_t::grouped_rows_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                                       uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, bool excluded,
-                                                       uint64_t* d_keys, float* d_dists, uint32_t* d_counts, uint32_t* d_computed,
-                                                       uint32_t* d_visited, cudaStream_t s) {
-    if (shards) return ERR_SHARDED;
-    if (char const* e = ensure_context()) return e;
-    if (nq == 0 || k == 0) return nullptr;
-    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
-    uint64_t entries = 0;
-    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, excluded ? EXCLUDED_GRAPH_SETS : GRAPH_SETS, &entries, s))
-        return e;
-
-    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
-        CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
-        CU(cudaStreamSynchronize(s));
-        return nullptr;
-    }
-    if (!groups) { /* one set: every query tests row 0 of the GROUPED kernel */
-        if (char const* e = group_upload.reserve(nq)) return e;
-        CU(cudaMemsetAsync(group_upload.ptr, 0, nq * 4, s));
-        groups = group_upload.ptr;
-    }
-    if (char const* e = ensure_key_table(s)) return e;
-    uint32_t const words = (uint32_t)((size + 31) / 32);
-    size_t const budget = (size_t)std::max(tune.group_bitmap_mb, 0) << 20;
-    size_t const per_round = std::min<size_t>(std::max<size_t>(budget / ((size_t)words * 4), 1), group_count);
-    size_t const rounds = (group_count + per_round - 1) / per_round;
-    if (char const* e = group_bits.reserve(per_round * words)) return e;
+/* graph: rows that allow the sets' slots, or (`excluded`) rows that allow every slot but them */
+char const* rows_search(frozen_index_t& ix, void const* d_queries, size_t nq, size_t stride, size_t k, key_sets_t const& sets, bool excluded,
+                        device_results_t const& out, cudaStream_t s) {
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
+    uint32_t const words = (uint32_t)((ix.size + 31) / 32);
+    size_t const budget = (size_t)std::max(ix.tune.group_bitmap_mb, 0) << 20;
+    size_t const per_round = std::min<size_t>(std::max<size_t>(budget / ((size_t)words * 4), 1), sets.count);
+    size_t const rounds = (sets.count + per_round - 1) / per_round;
+    if (char const* e = x.bits.reserve(per_round * words)) return e;
 
     launch_plan_t pl;
-    if (char const* e = plan((uint32_t)k, 0, pl, 0, true)) return e;
+    if (char const* e = ix.plan((uint32_t)k, 0, pl, 0, true)) return e;
     int const wpb = search_warps_per_block();
-    if (char const* e = h_status.reserve(nq)) return e;
-    if (char const* e = status.reserve(nq)) return e;
+    if (char const* e = ix.h_status.reserve(nq)) return e;
+    if (char const* e = ix.status.reserve(nq)) return e;
     /* the retry of a round scans every query id: the words of the other rounds' queries must read STATUS_OK */
-    CU(cudaMemsetAsync(status.ptr, 0, nq * 4, s));
-    if (profile_phases)
-        if (char const* e = phase_cycles.reserve(PHASE_COUNTERS)) return e;
+    CU(cudaMemsetAsync(ix.status.ptr, 0, nq * 4, s));
+    if (ix.profile_phases)
+        if (char const* e = ix.phase_cycles.reserve(PHASE_COUNTERS)) return e;
 
     /* the sets [g0, g1) into rows, then their queries: `items` work items, through `list` when it is not NULL */
     auto round = [&](uint32_t g0, uint32_t g1, uint32_t const* list, size_t items) -> char const* {
         /* allowed sets: rows of zeros that gain their slots; excluded sets: rows of ones that lose theirs */
-        CU(cudaMemsetAsync(group_bits.ptr, excluded ? 0xFF : 0, (size_t)(g1 - g0) * words * 4, s));
+        CU(cudaMemsetAsync(x.bits.ptr, excluded ? 0xFF : 0, (size_t)(g1 - g0) * words * 4, s));
         if (excluded)
-            excluded_bits_kernel<<<stream.sm_count * 16, 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, set_keys, g0, g1, words,
-                                                                      group_bits.ptr);
+            excluded_bits_kernel<<<ix.stream.sm_count * 16, 256, 0, s>>>(ix.key_table.cells.ptr, ix.key_table.mask, sets.offsets, sets.keys, g0,
+                                                                         g1, words, x.bits.ptr);
         else
-            grouped_bits_kernel<<<stream.sm_count * 16, 256, 0, s>>>(key_table.cells.ptr, key_table.mask, offsets, set_keys, g0, g1,
-                                                                     free_key, d.deleted_bits, (uint32_t)size, words, group_bits.ptr);
+            grouped_bits_kernel<<<ix.stream.sm_count * 16, 256, 0, s>>>(ix.key_table.cells.ptr, ix.key_table.mask, sets.offsets, sets.keys, g0,
+                                                                        g1, ix.free_key, ix.d.deleted_bits, (uint32_t)ix.size, words,
+                                                                        x.bits.ptr);
         CU(cudaGetLastError());
-        kernel_launches += 1;
+        ix.kernel_launches += 1;
         int const blocks = (int)std::min<size_t>((size_t)pl.blocks, (items + wpb - 1) / wpb);
         search_args_t a;
-        if (char const* e = prepare_launch(pl, (size_t)blocks * wpb, a, s)) return e;
+        if (char const* e = ix.prepare_launch(pl, (size_t)blocks * wpb, a, s)) return e;
         a.queries = static_cast<uint8_t const*>(d_queries);
         a.query_stride = stride;
         a.nq = (uint32_t)items;
         a.query_list = list;
         a.k = (uint32_t)k;
-        a.out_keys = d_keys;
-        a.out_dists = d_dists;
-        a.out_counts = d_counts;
-        a.out_computed = d_computed;
-        a.out_visited = d_visited;
-        a.status = status.ptr;
-        a.allow_bits = group_bits.ptr;
-        a.allow_groups = groups;
+        a.out_keys = out.keys;
+        a.out_dists = out.dists;
+        a.out_counts = out.counts;
+        a.out_computed = out.computed;
+        a.out_visited = out.visited;
+        a.status = ix.status.ptr;
+        a.allow_bits = x.bits.ptr;
+        a.allow_groups = sets.groups;
         a.allow_group_base = g0;
         a.allow_words = words;
-        if (profile_phases) a.phase_cycles = phase_cycles.ptr;
-        CU(cudaMemsetAsync(work_counter.ptr, 0, 8, s));
-        CU(cudaEventRecord(ev_begin, s));
-        CU(search_launch(d, a, blocks, pl.smem_per_block, s));
-        CU(cudaEventRecord(ev_end, s));
-        kernel_launches += 1;
-        CU(cudaMemcpyAsync(h_status.ptr, status.ptr, nq * 4, cudaMemcpyDeviceToHost, s));
+        if (ix.profile_phases) a.phase_cycles = ix.phase_cycles.ptr;
+        CU(cudaMemsetAsync(ix.work_counter.ptr, 0, 8, s));
+        CU(cudaEventRecord(ix.ev_begin, s));
+        CU(search_launch(ix.d, a, blocks, pl.smem_per_block, s));
+        CU(cudaEventRecord(ix.ev_end, s));
+        ix.kernel_launches += 1;
+        CU(cudaMemcpyAsync(ix.h_status.ptr, ix.status.ptr, nq * 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
-        CU(cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end));
+        CU(cudaEventElapsedTime(&ix.last_kernel_ms, ix.ev_begin, ix.ev_end));
         search_args_t every = a; /* the failed queries of this round, by query id */
         every.nq = (uint32_t)nq;
-        return retry_overflowed(every, pl.maxed, s);
+        return ix.retry_overflowed(every, pl.maxed, s);
     };
-    if (rounds == 1) return round(0, (uint32_t)group_count, nullptr, nq);
+    if (rounds == 1) return round(0, (uint32_t)sets.count, nullptr, nq);
 
     /* query ids sorted by set: round r serves the contiguous slice of ids whose sets lie in its range */
-    if (char const* e = group_ids.reserve(nq)) return e;
-    if (char const* e = group_order.reserve(nq)) return e;
-    if (char const* e = group_sorted.reserve(nq)) return e;
-    if (char const* e = group_bounds.reserve(rounds + 1)) return e;
-    iota_u32_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(group_ids.ptr, nq);
+    if (char const* e = x.bounds.reserve(rounds + 1)) return e;
+    if (char const* e = sort_queries(ix, sets.groups, nq, bits_for(sets.count), s)) return e;
+    round_bounds_kernel<<<(unsigned)((rounds + 1 + 255) / 256), 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, (uint32_t)per_round, (uint32_t)rounds,
+                                                                             x.bounds.ptr);
     CU(cudaGetLastError());
-    int end_bit = 1;
-    while (end_bit < 32 && (group_count - 1) >> end_bit) ++end_bit;
-    size_t temp_bytes = 0;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, groups, group_sorted.ptr, group_ids.ptr, group_order.ptr, (int)nq, 0, end_bit, s));
-    if (char const* e = group_sort_temp.reserve(temp_bytes)) return e;
-    CU(cub::DeviceRadixSort::SortPairs(group_sort_temp.ptr, temp_bytes, groups, group_sorted.ptr, group_ids.ptr, group_order.ptr, (int)nq, 0,
-                                       end_bit, s));
-    round_bounds_kernel<<<(unsigned)((rounds + 1 + 255) / 256), 256, 0, s>>>(group_sorted.ptr, (uint32_t)nq, (uint32_t)per_round,
-                                                                             (uint32_t)rounds, group_bounds.ptr);
-    CU(cudaGetLastError());
-    kernel_launches += 3;
+    ix.kernel_launches += 3;
     std::vector<uint32_t> bounds(rounds + 1);
-    CU(cudaMemcpyAsync(bounds.data(), group_bounds.ptr, (rounds + 1) * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(bounds.data(), x.bounds.ptr, (rounds + 1) * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     for (size_t r = 0; r < rounds; ++r) {
         if (bounds[r + 1] == bounds[r]) continue; /* no query asks for these sets */
-        uint32_t const g0 = (uint32_t)(r * per_round), g1 = (uint32_t)std::min(group_count, (r + 1) * per_round);
-        if (char const* e = round(g0, g1, group_order.ptr + bounds[r], bounds[r + 1] - bounds[r])) return e;
+        uint32_t const g0 = (uint32_t)(r * per_round), g1 = (uint32_t)std::min(sets.count, (r + 1) * per_round);
+        if (char const* e = round(g0, g1, x.order.ptr + bounds[r], bounds[r + 1] - bounds[r])) return e;
     }
     return nullptr;
 }
 
-/* host queries of any kind, host sets and host outputs: the sets checked here, then uploaded and run through the device path */
-char const* frozen_index_t::grouped_filtered_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                                         uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                         uint64_t const* set_keys, host_results_t const& out, size_t* total) {
-    std::lock_guard<std::mutex> lock(mutex);
-    if (shards) return ERR_SHARDED;
-    if (nq == 0 || k == 0) return nullptr;
-    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, GRAPH_SETS)) return e;
-    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
-    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
-                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
-        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
-        return grouped_filtered_search_device(dq, nq, vs, k, group_upload.ptr, group_offsets.ptr, group_count, key_stage.ptr, r.keys, r.dists,
-                                              r.counts, r.computed, r.visited, stream);
-    });
-}
-
-/* the same for excluded sets; `groups` may be NULL with one set */
-char const* frozen_index_t::grouped_excluded_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                                         uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                         uint64_t const* set_keys, host_results_t const& out, size_t* total) {
-    std::lock_guard<std::mutex> lock(mutex);
-    if (shards) return ERR_SHARDED;
-    if (nq == 0 || k == 0) return nullptr;
-    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, EXCLUDED_GRAPH_SETS)) return e;
-    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
-    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
-                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
-        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
-        return grouped_excluded_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count, key_stage.ptr,
-                                              r.keys, r.dists, r.counts, r.computed, r.visited, stream);
-    });
-}
-
-/* ---------------------------------------------------------------------------------------------- */
-/*  exact filtered search: search_exact_ over the live slots of each query's key set              */
-/* ---------------------------------------------------------------------------------------------- */
-
-size_t frozen_index_t::exact_filter_scratch_t::bytes() const {
-    return entry_counts.capacity * 8 + entry_at.capacity * 8 + words.capacity * 8 + words_sorted.capacity * 8 + rows.capacity * 4 +
-           list_at.capacity * 4 + query_at.capacity * 4 + per_set.capacity * 4 + item_at.capacity * 4 + items.capacity * sizeof(exact_item_t) +
-           order.capacity * 4 + sorted.capacity * 4 + ids.capacity * 4 + groups.capacity * 4 + scalars.capacity * 4 + temp.capacity +
-           buckets.capacity * 4 + bucket_at.capacity * 4 +
-           queries.capacity + keys.capacity * 8 + dists.capacity * 4 + counts.capacity * 4 + exact.capacity;
-}
-
-namespace {
-
 /* the slot-list build, step 1: the live slots of every entry, placed by an exclusive scan into x.entry_at (one extra zero
  * count: its place, entry_at[n_entries], is the cell total). Nothing waits. */
 char const* listed_place_cells(frozen_index_t& ix, uint64_t const* set_keys, size_t n_entries, cudaStream_t s) {
-    frozen_index_t::exact_filter_scratch_t& x = ix.exact_filter;
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
     size_t temp_bytes = 0;
     if (char const* e = x.entry_counts.reserve(n_entries + 1)) return e;
     if (char const* e = x.entry_at.reserve(n_entries + 1)) return e;
@@ -544,7 +442,7 @@ char const* listed_place_cells(frozen_index_t& ix, uint64_t const* set_keys, siz
  * the bits in use and deduplicated, leave set g's ascending, duplicate-free slots at x.rows[x.list_at[g] .. x.list_at[g + 1]) */
 char const* listed_build_lists(frozen_index_t& ix, uint64_t const* offsets, uint32_t sets, uint64_t const* set_keys, size_t n_entries,
                                uint64_t cells, cudaStream_t s) {
-    frozen_index_t::exact_filter_scratch_t& x = ix.exact_filter;
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
     auto temp_for = [&](size_t bytes) { return x.temp.reserve(std::max<size_t>(bytes, 1)); };
     size_t temp_bytes = 0;
     int const n_cells = (int)cells;
@@ -573,88 +471,57 @@ char const* listed_build_lists(frozen_index_t& ix, uint64_t const* offsets, uint
     return nullptr;
 }
 
-} // namespace
-
-char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, uint32_t const* groups,
-                                                        uint64_t const* offsets, size_t group_count, uint64_t const* set_keys, uint64_t* d_keys,
-                                                        float* d_dists, uint32_t* d_counts, uint32_t* d_computed, uint32_t* d_visited,
-                                                        cudaStream_t s) {
-    if (shards) return ERR_SHARDED;
-    if (char const* e = ensure_context()) return e;
-    if (nq == 0 || k == 0) return nullptr;
-    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
-    uint64_t entries = 0;
-    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, EXACT_SETS, &entries, s)) return e;
-    exact_filter_scratch_t& x = exact_filter;
-
-    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
-        CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
-        CU(cudaStreamSynchronize(s));
-        return nullptr;
-    }
-    uint32_t qpc = 0;
-    if (char const* e = exact_listed_queries_per_item(d, k, &qpc)) return e;
-    if (char const* e = ensure_key_table(s)) return e;
-    uint32_t const sets = (uint32_t)group_count;
+/* exact, allowed sets: search_exact_ over the live slots of each query's set, `entries` keys in all the sets, `qpc` queries
+ * per work item of the LISTED kernel */
+char const* listed_exact_search(frozen_index_t& ix, void const* d_queries, size_t nq, size_t stride, size_t k, key_sets_t const& sets,
+                                uint64_t entries, uint32_t qpc, device_results_t const& out, cudaStream_t s) {
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
+    uint32_t const n_sets = (uint32_t)sets.count;
     size_t const n_entries = (size_t)entries;
     auto temp_for = [&](size_t bytes) { return x.temp.reserve(std::max<size_t>(bytes, 1)); };
     size_t temp_bytes = 0;
 
     /* 1. the live slots of every entry, placed by an exclusive scan */
-    if (char const* e = listed_place_cells(*this, set_keys, n_entries, s)) return e;
+    if (char const* e = listed_place_cells(ix, sets.keys, n_entries, s)) return e;
     /* 2. the queries sorted by set, cut into work items of at most qpc queries that never mix sets (counted here, written
      * once the lists are placed) */
-    if (char const* e = x.groups.reserve(nq)) return e;
-    if (char const* e = x.ids.reserve(nq)) return e;
-    if (char const* e = x.order.reserve(nq)) return e;
-    if (char const* e = x.sorted.reserve(nq)) return e;
-    if (char const* e = x.query_at.reserve(group_count + 1)) return e;
-    if (char const* e = x.per_set.reserve(group_count + 1)) return e;
-    if (char const* e = x.item_at.reserve(group_count + 1)) return e;
+    if (char const* e = x.query_at.reserve(sets.count + 1)) return e;
+    if (char const* e = x.per_set.reserve(sets.count + 1)) return e;
+    if (char const* e = x.item_at.reserve(sets.count + 1)) return e;
     if (char const* e = x.items.reserve(nq)) return e;
-    if (!groups) { /* one set: every query uses set 0 */
-        CU(cudaMemsetAsync(x.groups.ptr, 0, nq * 4, s));
-        groups = x.groups.ptr;
-    }
-    iota_u32_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(x.ids.ptr, nq);
+    if (char const* e = sort_queries(ix, sets.groups, nq, bits_for(sets.count), s)) return e;
+    listed_item_counts_kernel<<<grid_for(sets.count + 1, ix.stream.sm_count), 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, n_sets, qpc,
+                                                                                           x.query_at.ptr, x.per_set.ptr);
     CU(cudaGetLastError());
-    int group_bits = 1;
-    while (group_bits < 32 && (group_count - 1) >> group_bits) ++group_bits;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, groups, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, group_bits, s));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp_bytes, x.per_set.ptr, x.item_at.ptr, (int)(sets.count + 1), s));
     if (char const* e = temp_for(temp_bytes)) return e;
-    CU(cub::DeviceRadixSort::SortPairs(x.temp.ptr, temp_bytes, groups, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, group_bits, s));
-    listed_item_counts_kernel<<<grid_for(group_count + 1, stream.sm_count), 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, sets, qpc, x.query_at.ptr,
-                                                                                         x.per_set.ptr);
-    CU(cudaGetLastError());
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp_bytes, x.per_set.ptr, x.item_at.ptr, (int)(group_count + 1), s));
-    if (char const* e = temp_for(temp_bytes)) return e;
-    CU(cub::DeviceScan::ExclusiveSum(x.temp.ptr, temp_bytes, x.per_set.ptr, x.item_at.ptr, (int)(group_count + 1), s));
+    CU(cub::DeviceScan::ExclusiveSum(x.temp.ptr, temp_bytes, x.per_set.ptr, x.item_at.ptr, (int)(sets.count + 1), s));
     /* one read-back: the cell total sizes the lists and the item count the grid. The total is an exact 64-bit sum (the
      * counts are 64-bit), so a multi index whose sets name more than INT_MAX cells is refused here, before the sort (whose
      * item count is an int) or any write to the lists. */
     uint64_t cells = 0;
     uint32_t n_items = 0;
     CU(cudaMemcpyAsync(&cells, x.entry_at.ptr + n_entries, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&n_items, x.item_at.ptr + group_count, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&n_items, x.item_at.ptr + sets.count, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (cells > 0x7FFFFFFFull) return "Too many listed rows in one call";
 
     /* 3. (set << 32 | slot) words, sorted over the bits in use and deduplicated: per-set ascending slot lists */
-    if (char const* e = listed_build_lists(*this, offsets, sets, set_keys, n_entries, cells, s)) return e;
+    if (char const* e = listed_build_lists(ix, sets.offsets, n_sets, sets.keys, n_entries, cells, s)) return e;
 
-    listed_items_kernel<<<grid_for(group_count, stream.sm_count), 256, 0, s>>>(x.query_at.ptr, x.item_at.ptr, x.list_at.ptr, sets, qpc,
-                                                                               x.items.ptr);
+    listed_items_kernel<<<grid_for(sets.count, ix.stream.sm_count), 256, 0, s>>>(x.query_at.ptr, x.item_at.ptr, x.list_at.ptr, n_sets, qpc,
+                                                                                 x.items.ptr);
     CU(cudaGetLastError());
-    kernel_launches += 8;
+    ix.kernel_launches += 8;
 
     /* 4. the gathered batch through the listed scans and the unchanged merge, then back to the caller's order */
-    size_t const vs = d.vec_stride;
+    size_t const vs = ix.d.vec_stride;
     if (char const* e = x.queries.reserve(nq * vs)) return e;
     if (char const* e = x.keys.reserve(nq * k)) return e;
     if (char const* e = x.dists.reserve(nq * k)) return e;
     if (char const* e = x.counts.reserve(nq)) return e;
     listed_gather_queries_kernel<<<(unsigned)std::min<size_t>(nq, 65535), 128, 0, s>>>(static_cast<uint8_t const*>(d_queries), stride,
-                                                                                       x.order.ptr, (uint32_t)nq, (uint32_t)d.bytes_per_vector,
+                                                                                       x.order.ptr, (uint32_t)nq, (uint32_t)ix.d.bytes_per_vector,
                                                                                        (uint32_t)vs, x.queries.ptr);
     CU(cudaGetLastError());
     exact_listed_t listed;
@@ -662,103 +529,53 @@ char const* frozen_index_t::grouped_exact_search_device(void const* d_queries, s
     listed.n_items = n_items;
     listed.rows = x.rows.ptr;
     listed.total_rows = (uint32_t)cells; /* the lists' rows, duplicates still counted: the planner's bound */
-    CU(cudaEventRecord(ev_begin, s));
-    if (char const* e = exact_listed_search_device(d, stream.sm_count, x.queries.ptr, nq, k, listed, x.keys.ptr, x.dists.ptr, x.counts.ptr,
-                                                   x.exact, s))
+    CU(cudaEventRecord(ix.ev_begin, s));
+    if (char const* e = exact_listed_search_device(ix.d, ix.stream.sm_count, x.queries.ptr, nq, k, listed, x.keys.ptr, x.dists.ptr,
+                                                   x.counts.ptr, x.exact, s))
         return e;
-    CU(cudaEventRecord(ev_end, s));
+    CU(cudaEventRecord(ix.ev_end, s));
     listed_scatter_kernel<<<(unsigned)std::min<size_t>(nq, 65535), 128, 0, s>>>(x.order.ptr, x.sorted.ptr, x.list_at.ptr, (uint32_t)nq,
-                                                                                (uint32_t)k, x.keys.ptr, x.dists.ptr, x.counts.ptr, d_keys,
-                                                                                d_dists, d_counts, d_computed, d_visited);
+                                                                                (uint32_t)k, x.keys.ptr, x.dists.ptr, x.counts.ptr, out.keys,
+                                                                                out.dists, out.counts, out.computed, out.visited);
     CU(cudaGetLastError());
-    kernel_launches += 4;
+    ix.kernel_launches += 4;
     CU(cudaStreamSynchronize(s));
-    CU(cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end));
+    CU(cudaEventElapsedTime(&ix.last_kernel_ms, ix.ev_begin, ix.ev_end));
     return nullptr;
 }
 
-/* host queries of any kind, host sets and host outputs, as grouped_filtered_search_host serves them */
-char const* frozen_index_t::grouped_exact_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                                      uint32_t const* groups, uint64_t const* offsets, size_t group_count, uint64_t const* set_keys,
-                                                      host_results_t const& out, size_t* total) {
-    std::lock_guard<std::mutex> lock(mutex);
-    if (shards) return ERR_SHARDED;
-    if (nq == 0 || k == 0) return nullptr;
-    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, EXACT_SETS)) return e;
-    if (!loaded || d.n == 0) return answer_empty(nq, k, out);
-    return search_round_trip(q, nq, stride, query_scalar, k, out, total,
-                             [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
-        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
-        return grouped_exact_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count, key_stage.ptr,
-                                           r.keys, r.dists, r.counts, r.computed, nullptr, stream);
-    });
-}
-
-/* ---------------------------------------------------------------------------------------------- */
-/*  exact excluded search: search_exact_ over the live slots outside each query's key set         */
-/* ---------------------------------------------------------------------------------------------- */
-
-/* The scan order (distance ascending, slot descending) is total, so the k best entries outside a set of e live slots are
- * what remains of the unfiltered top-(k + e) once the set's slots are dropped. The sets become slot lists (the exact
- * filtered search's build); the queries are bucketed by k + e rounded up to a power of two, and each bucket runs the
- * unfiltered scan once at its count, with slots for keys, then the drop. */
-char const* frozen_index_t::grouped_excluded_exact_search_device(void const* d_queries, size_t nq, size_t stride, size_t k,
-                                                                 uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                                 uint64_t const* set_keys, uint64_t* d_keys, float* d_dists, uint32_t* d_counts,
-                                                                 uint32_t* d_computed, uint32_t* d_visited, cudaStream_t s) {
-    if (shards) return ERR_SHARDED;
-    if (char const* e = ensure_context()) return e;
-    if (nq == 0 || k == 0) return nullptr;
-    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
-    uint64_t entries = 0;
-    if (char const* e = check_key_sets_device(*this, groups, nq, offsets, group_count, EXACT_SETS, &entries, s)) return e;
-    exact_filter_scratch_t& x = exact_filter;
-
-    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
-        CU(search_fill_empty(d_keys, d_dists, d_counts, d_computed, d_visited, nq, k, s));
-        CU(cudaStreamSynchronize(s));
-        return nullptr;
-    }
-    if (char const* e = exact_search_check(d, k)) return e; /* the refusals of search(exact = true) at this count */
-    if (char const* e = ensure_key_table(s)) return e;
-    uint32_t const sets = (uint32_t)group_count;
+/* exact, excluded sets: search_exact_ over the live slots outside each query's set. The scan order (distance ascending,
+ * slot descending) is total, so the k best entries outside a set of e live slots are what remains of the unfiltered
+ * top-(k + e) once the set's slots are dropped. The sets become slot lists (the exact filtered search's build); the
+ * queries are bucketed by k + e rounded up to a power of two, and each bucket runs the unfiltered scan once at its count,
+ * with slots for keys, then the drop. */
+char const* excluded_exact_search(frozen_index_t& ix, void const* d_queries, size_t nq, size_t stride, size_t k, key_sets_t const& sets,
+                                  uint64_t entries, device_results_t const& out, cudaStream_t s) {
+    frozen_index_t::key_set_scratch_t& x = ix.key_set_scratch;
     size_t const n_entries = (size_t)entries;
 
     /* 1. the sets' live slots as sorted lists */
-    if (char const* e = listed_place_cells(*this, set_keys, n_entries, s)) return e;
+    if (char const* e = listed_place_cells(ix, sets.keys, n_entries, s)) return e;
     uint64_t cells = 0;
     CU(cudaMemcpyAsync(&cells, x.entry_at.ptr + n_entries, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (cells > 0x7FFFFFFFull) return "Too many listed rows in one call";
-    if (char const* e = listed_build_lists(*this, offsets, sets, set_keys, n_entries, cells, s)) return e;
+    if (char const* e = listed_build_lists(ix, sets.offsets, (uint32_t)sets.count, sets.keys, n_entries, cells, s)) return e;
 
     /* 2. the queries bucketed by the count their scan needs, in query order within a bucket (the sort is stable). No count
      * past max(k, live) is needed: that many rows hold every live entry. */
-    uint64_t const live = size - count_deleted, cap = std::max<uint64_t>(k, live);
+    uint64_t const live = ix.size - ix.count_deleted, cap = std::max<uint64_t>(k, live);
     int constexpr BUCKETS = 64;
-    if (char const* e = x.groups.reserve(nq)) return e;
-    if (char const* e = x.ids.reserve(nq)) return e;
-    if (char const* e = x.order.reserve(nq)) return e;
-    if (char const* e = x.sorted.reserve(nq)) return e;
     if (char const* e = x.buckets.reserve(nq)) return e;
-    if (char const* e = x.bucket_at.reserve(BUCKETS + 1)) return e;
-    if (!groups) { /* one set: every query uses set 0 */
-        CU(cudaMemsetAsync(x.groups.ptr, 0, nq * 4, s));
-        groups = x.groups.ptr;
-    }
-    excluded_bucket_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(groups, x.list_at.ptr, (uint32_t)nq, k, cap, x.buckets.ptr);
+    if (char const* e = x.bounds.reserve(BUCKETS + 1)) return e;
+    excluded_bucket_kernel<<<grid_for(nq, ix.stream.sm_count), 256, 0, s>>>(sets.groups, x.list_at.ptr, (uint32_t)nq, k, cap, x.buckets.ptr);
     CU(cudaGetLastError());
-    iota_u32_kernel<<<grid_for(nq, stream.sm_count), 256, 0, s>>>(x.ids.ptr, nq);
+    if (char const* e = sort_queries(ix, x.buckets.ptr, nq, 6, s)) return e;
+    round_bounds_kernel<<<1, 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, 1, BUCKETS, x.bounds.ptr);
     CU(cudaGetLastError());
-    size_t temp_bytes = 0;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, x.buckets.ptr, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, 6, s));
-    if (char const* e = x.temp.reserve(std::max<size_t>(temp_bytes, 1))) return e;
-    CU(cub::DeviceRadixSort::SortPairs(x.temp.ptr, temp_bytes, x.buckets.ptr, x.sorted.ptr, x.ids.ptr, x.order.ptr, (int)nq, 0, 6, s));
-    round_bounds_kernel<<<1, 256, 0, s>>>(x.sorted.ptr, (uint32_t)nq, 1, BUCKETS, x.bucket_at.ptr);
-    CU(cudaGetLastError());
-    kernel_launches += 4;
+    ix.kernel_launches += 4;
     std::vector<uint32_t> at(BUCKETS + 1);
-    CU(cudaMemcpyAsync(at.data(), x.bucket_at.ptr, (BUCKETS + 1) * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(at.data(), x.bounds.ptr, (BUCKETS + 1) * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     auto count_of = [&](int b) { return std::min<uint64_t>(1ull << b, cap); };
     uint64_t widest = 0;
@@ -769,53 +586,91 @@ char const* frozen_index_t::grouped_excluded_exact_search_device(void const* d_q
             rows = std::max<size_t>(rows, (size_t)(at[b + 1] - at[b]) * widest);
         }
     /* count > 256 past the tiled stage is refused here, before any output is written */
-    if (char const* e = exact_search_check(d, widest)) return e;
+    if (char const* e = exact_search_check(ix.d, widest)) return e;
 
     /* 3. the batch gathered in bucket order; per bucket the unfiltered scan at its count, then the drop into caller order */
-    size_t const vs = d.vec_stride;
+    size_t const vs = ix.d.vec_stride;
     if (char const* e = x.queries.reserve(nq * vs)) return e;
     if (char const* e = x.keys.reserve(rows)) return e;
     if (char const* e = x.dists.reserve(rows)) return e;
     if (char const* e = x.counts.reserve(nq)) return e;
     listed_gather_queries_kernel<<<(unsigned)std::min<size_t>(nq, 65535), 128, 0, s>>>(static_cast<uint8_t const*>(d_queries), stride,
-                                                                                       x.order.ptr, (uint32_t)nq, (uint32_t)d.bytes_per_vector,
+                                                                                       x.order.ptr, (uint32_t)nq, (uint32_t)ix.d.bytes_per_vector,
                                                                                        (uint32_t)vs, x.queries.ptr);
     CU(cudaGetLastError());
-    kernel_launches += 1;
-    CU(cudaEventRecord(ev_begin, s));
+    ix.kernel_launches += 1;
+    CU(cudaEventRecord(ix.ev_begin, s));
     for (int b = 0; b < BUCKETS; ++b) {
         uint32_t const q0 = at[b], n_b = at[b + 1] - at[b];
         if (!n_b) continue;
         uint64_t const width = count_of(b);
-        if (char const* e = exact_search_device(d, stream.sm_count, x.queries.ptr + (size_t)q0 * vs, n_b, vs, width, false, true, x.keys.ptr,
-                                                x.dists.ptr, x.counts.ptr, x.exact, s))
+        if (char const* e = exact_search_device(ix.d, ix.stream.sm_count, x.queries.ptr + (size_t)q0 * vs, n_b, vs, width, false, true,
+                                                x.keys.ptr, x.dists.ptr, x.counts.ptr, x.exact, s))
             return e;
-        excluded_drop_kernel<<<(n_b + 7) / 8, 256, 0, s>>>(x.order.ptr + q0, groups, x.list_at.ptr, x.rows.ptr, n_b, (uint32_t)width,
-                                                           (uint32_t)k, x.keys.ptr, x.dists.ptr, x.counts.ptr, d.keys, (uint32_t)live, d_keys,
-                                                           d_dists, d_counts, d_computed, d_visited);
+        excluded_drop_kernel<<<(n_b + 7) / 8, 256, 0, s>>>(x.order.ptr + q0, sets.groups, x.list_at.ptr, x.rows.ptr, n_b, (uint32_t)width,
+                                                           (uint32_t)k, x.keys.ptr, x.dists.ptr, x.counts.ptr, ix.d.keys, (uint32_t)live,
+                                                           out.keys, out.dists, out.counts, out.computed, out.visited);
         CU(cudaGetLastError());
-        kernel_launches += 3;
+        ix.kernel_launches += 3;
     }
-    CU(cudaEventRecord(ev_end, s));
+    CU(cudaEventRecord(ix.ev_end, s));
     CU(cudaStreamSynchronize(s));
-    CU(cudaEventElapsedTime(&last_kernel_ms, ev_begin, ev_end));
+    CU(cudaEventElapsedTime(&ix.last_kernel_ms, ix.ev_begin, ix.ev_end));
     return nullptr;
 }
 
-/* host queries of any kind, host sets and host outputs, as grouped_exact_search_host serves them */
-char const* frozen_index_t::grouped_excluded_exact_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
-                                                               uint32_t const* groups, uint64_t const* offsets, size_t group_count,
-                                                               uint64_t const* set_keys, host_results_t const& out, size_t* total) {
+} // namespace
+
+size_t frozen_index_t::key_set_scratch_t::bytes() const {
+    return bits.capacity * 4 + flag.capacity * 4 + groups.capacity * 4 + offsets.capacity * 8 + ids.capacity * 4 + order.capacity * 4 +
+           sorted.capacity * 4 + bounds.capacity * 4 + temp.capacity + entry_counts.capacity * 8 + entry_at.capacity * 8 +
+           words.capacity * 8 + words_sorted.capacity * 8 + rows.capacity * 4 + list_at.capacity * 4 + query_at.capacity * 4 +
+           per_set.capacity * 4 + item_at.capacity * 4 + items.capacity * sizeof(exact_item_t) + scalars.capacity * 4 +
+           buckets.capacity * 4 + queries.capacity + keys.capacity * 8 + dists.capacity * 4 + counts.capacity * 4 + exact.capacity;
+}
+
+char const* frozen_index_t::key_set_search_device(void const* d_queries, size_t nq, size_t stride, size_t k, key_sets_t const& sets,
+                                                  bool excluded, bool exact, device_results_t const& out, cudaStream_t s) {
+    if (shards) return ERR_SHARDED;
+    if (char const* e = ensure_context()) return e;
+    if (nq == 0 || k == 0) return nullptr;
+    if (nq > 0x7FFFFFFFull) return "Too many queries in one batch";
+    uint64_t entries = 0;
+    if (char const* e = check_key_sets_device(*this, sets, nq, rules_of(excluded, exact), &entries, s)) return e;
+    if (!loaded || d.n == 0) { /* no matches, no error (index.hpp:3036-3037) */
+        CU(search_fill_empty(out.keys, out.dists, out.counts, out.computed, out.visited, nq, k, s));
+        CU(cudaStreamSynchronize(s));
+        return nullptr;
+    }
+    /* the exact forms' refusals at this count, before the key table is built */
+    uint32_t qpc = 0;
+    if (exact)
+        if (char const* e = excluded ? exact_search_check(d, k) : exact_listed_queries_per_item(d, k, &qpc)) return e;
+    key_sets_t in = sets;
+    if (!in.groups) { /* one set: every query uses set 0 */
+        if (char const* e = key_set_scratch.groups.reserve(nq)) return e;
+        CU(cudaMemsetAsync(key_set_scratch.groups.ptr, 0, nq * 4, s));
+        in.groups = key_set_scratch.groups.ptr;
+    }
+    if (char const* e = ensure_key_table(s)) return e;
+    if (!exact) return rows_search(*this, d_queries, nq, stride, k, in, excluded, out, s);
+    if (!excluded) return listed_exact_search(*this, d_queries, nq, stride, k, in, entries, qpc, out, s);
+    return excluded_exact_search(*this, d_queries, nq, stride, k, in, entries, out, s);
+}
+
+/* host queries of any kind, host sets and host outputs: the sets checked here, then uploaded and run through the device path */
+char const* frozen_index_t::key_set_search_host(void const* q, size_t nq, size_t stride, uint32_t query_scalar, size_t k,
+                                                key_sets_t const& sets, bool excluded, bool exact, host_results_t const& out, size_t* total) {
     std::lock_guard<std::mutex> lock(mutex);
     if (shards) return ERR_SHARDED;
     if (nq == 0 || k == 0) return nullptr;
-    if (char const* e = check_key_sets_host(groups, nq, offsets, group_count, EXACT_SETS)) return e;
+    if (char const* e = check_key_sets_host(sets, nq, rules_of(excluded, exact))) return e;
     if (!loaded || d.n == 0) return answer_empty(nq, k, out);
     return search_round_trip(q, nq, stride, query_scalar, k, out, total,
                              [&](void const* dq, size_t vs, device_results_t const& r) -> char const* {
-        if (char const* e = upload_key_sets(*this, groups, nq, offsets, group_count, set_keys)) return e;
-        return grouped_excluded_exact_search_device(dq, nq, vs, k, groups ? group_upload.ptr : nullptr, group_offsets.ptr, group_count,
-                                                    key_stage.ptr, r.keys, r.dists, r.counts, r.computed, nullptr, stream);
+        if (char const* e = upload_key_sets(*this, sets, nq)) return e;
+        key_sets_t const uploaded{sets.groups ? key_set_scratch.groups.ptr : nullptr, key_set_scratch.offsets.ptr, sets.count, key_stage.ptr};
+        return key_set_search_device(dq, nq, vs, k, uploaded, excluded, exact, r, stream);
     });
 }
 
